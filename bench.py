@@ -44,7 +44,14 @@ def parse():
   p.add_argument("--no-graph", action="store_true", help="launch kernels directly instead of replaying a CUDA graph")
   p.add_argument("--cpu-sample-worlds", type=int, default=None)
   p.add_argument("--no-cpu", action="store_true", help="skip the cpu_baseline leg (kernel A/B sweeps)")
-  return p.parse_args()
+  p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                 help="write the last timed step's outputs (qpos, qvel, qacc, ...) to DIR/<field>.npy")
+  a = p.parse_args()
+  if a.steps < 1 or a.warmup < 0:
+    p.error("--steps must be >= 1 and --warmup >= 0")
+  if a.dump_outputs and a.impl != "ours":
+    p.error("--dump-outputs writes the GPU arm's outputs; --impl reference has none")
+  return a
 
 
 def usable_cores() -> int:
@@ -63,7 +70,7 @@ def usable_cores() -> int:
 
 
 class ClockSampler:
-  """Samples nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md clocks line)."""
+  """Samples nvidia-smi clocks / throttle reasons during the timed region."""
 
   Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -101,6 +108,37 @@ class ClockSampler:
           if v.lower().startswith("active"):
             reasons.add(n)
     return {"sm_mhz": float(np.median(sm)) if sm else None, "sm_max_mhz": max(mx) if mx else None, "reasons": sorted(reasons), "samples": len(sm)}
+
+
+def gpu_info(gpu_index):
+  """Name and power limit of the card the line was measured on (part of every absolute number it reports)."""
+  try:
+    out = subprocess.run(["nvidia-smi", f"--id={gpu_index}", "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                         capture_output=True, text=True, timeout=30).stdout.strip().split(", ")
+    return {"name": out[0], "power_limit_w": float(out[1])}
+  except Exception:
+    return {"name": None, "power_limit_w": None}
+
+
+# --------------------------------------------------------------------------------------------- output dump
+
+# What a caller of step(m, d) reads back: the advanced state, its accelerations and constraint forces, the solver's row count.
+DUMP_FIELDS = ("qpos", "qvel", "act", "ctrl", "time", "qacc", "qacc_warmstart", "qfrc_constraint", "sensordata", "nefc", "solver_niter")
+DUMP_LIMIT = 64 * 2**20
+
+
+def collect_outputs(d, nworld):
+  """DUMP_FIELDS as float32 (counters as float64); above DUMP_LIMIT a seeded sample of worlds, indices in `world_index`."""
+  ts = {n: getattr(d, n) for n in DUMP_FIELDS if getattr(d, n).numel()}
+  per_world = sum((t.numel() // nworld) * (4 if t.is_floating_point() else 8) for t in ts.values())
+  out = {}
+  if per_world * nworld > DUMP_LIMIT:
+    idx = np.sort(np.random.default_rng(0).choice(nworld, size=DUMP_LIMIT // (per_world + 8), replace=False))
+    out["world_index"] = idx.astype(np.float64)
+    ts = {n: t[idx] for n, t in ts.items()}
+  for n, t in ts.items():
+    out[n] = t.cpu().numpy().astype(np.float32 if t.is_floating_point() else np.float64)
+  return out
 
 
 # --------------------------------------------------------------------------------------------- algorithmic bytes
@@ -211,6 +249,8 @@ def run_reference(args):
 
 # --------------------------------------------------------------------------------------------- GPU arm
 
+HBM_PEAK_GBS = 3350.0  # H100 SXM data sheet (HBM3); the roofline's denominator
+
 
 def run_ours(args):
   import torch
@@ -243,8 +283,9 @@ def run_ours(args):
   center = torch.from_numpy(np.asarray(mjd.ctrl, dtype=np.float32)).cuda()
   traj = torch.from_numpy(np.asarray(ctrls, dtype=np.float32)).cuda() if ctrls is not None else None  # (nstep, nu), device resident
   data_mb = sum(t.numel() * t.element_size() for o in (d, d.efc, d.contact) for t in vars(o).values() if isinstance(t, torch.Tensor)) / 2**20
-  # timing rule: a per-step working set below the 126 MB L2 is flushed between timed steps (each step then gets its own event pair)
-  flush = torch.empty(256 * 2**20 // 4, dtype=torch.float32, device="cuda") if data_mb <= 126 else None
+  # timing rule: a per-step working set that fits the L2 (50 MB on an H100) is flushed between timed steps (each step then gets its own event pair)
+  l2_mb = torch.cuda.get_device_properties(local).L2_cache_size / 2**20
+  flush = torch.empty(256 * 2**20 // 4, dtype=torch.float32, device="cuda") if data_mb <= l2_mb else None
   # ranks use shifted Halton step indices so their noise streams differ
   world_offset = rank * nworld
 
@@ -325,6 +366,7 @@ def run_ours(args):
       stream.synchronize()
       ms = sum(a.elapsed_time(b) for a, b in evs)
     barrier()
+    outputs = collect_outputs(d, nworld) if args.dump_outputs and rank == 0 else None
     # ---- statistics of the run (untimed), taken from the last timed step
     ncon_mean = float(d.nacon.cpu()[0]) / nworld
     nefc_mean = float(d.nefc.float().mean().cpu())
@@ -428,32 +470,15 @@ def run_ours(args):
   e2e_value = shard.whole_job_rate(nworld * e2e_steps, e2e_ms_max * 1e-3, world)
 
   if rank == 0:
-    peaks = {}
-    try:
-      peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
-    except Exception:
-      pass
-    peak = float(peaks.get("hbm_gbs", 6650.0))
+    if outputs is not None:
+      os.makedirs(args.dump_outputs, exist_ok=True)
+      for n, v in outputs.items():
+        np.save(os.path.join(args.dump_outputs, n + ".npy"), v)
+    peak = HBM_PEAK_GBS
     words = algorithmic_words(mjm, tabs, ncon_mean, nefc_mean, m.nv_pad)
     top = max(kms, key=kms.get)
     bytes_launch = 4.0 * words[top] * nworld
     achieved = bytes_launch / (kms[top] * 1e-3) / 1e9
-    traffic, issue = None, None
-    try:  # DRAM bytes of the same kernel from the committed `ncu --set full` capture (profiles/r02_kernels.md); humanoid only
-      if args.workload == "humanoid":
-        prof = json.load(open(os.path.join(ROOT, "profiles", "r02_traffic.json")))
-        traffic = prof["traffic_bytes"].get("k_" + top)
-        traffic = traffic * nworld / 8192.0 if traffic is not None else None
-        # second roofline (context; the kernels are issue / latency bound, DESIGN.md section 3): warp instructions of the same capture
-        # against the SM's issue rate -- 148 SMs x 4 schedulers x one warp instruction per cycle at the SM clock sampled under load
-        winst = prof.get("warp_inst", {}).get("k_" + top)
-        mhz = float((clocks or {}).get("sm_mhz") or 0.0)
-        if winst and mhz > 0:
-          rate = winst * nworld / 8192.0 / (kms[top] * 1e-3)
-          issue = {"warp_inst_per_launch": winst * nworld / 8192.0, "achieved_warp_inst_per_s": rate, "peak_warp_inst_per_s": 148 * 4 * mhz * 1e6,
-                   "frac": rate / (148 * 4 * mhz * 1e6), "source": "smsp__inst_executed.sum of profiles/r02_kernels.md"}
-    except Exception:
-      pass
     step_bytes = 4.0 * sum(words.values()) * nworld
     cpu = None
     if world == 1 and not args.no_cpu:  # reported baseline, rank 0 at N = 1 only: a bounded sample of the same workload on the host cores
@@ -469,7 +494,7 @@ def run_ours(args):
       "dtype": "f32", "data": "synthetic",
       "config": {
         "workload": wl["label"] if nworld == wl["nworld"] else wl["label"].replace(f"nworld={wl['nworld']}", f"nworld={nworld}"),
-        "cuda_graph": graph is not None, "l2": f"per-step Data working set ({data_mb:.0f} MB of Data tensors at {nworld} worlds) exceeds the 126 MB L2; no explicit flush" if data_mb > 126 else f"Data tensors are {data_mb:.0f} MB (< 126 MB L2): 256 MB scratch buffer written between timed steps",
+        "cuda_graph": graph is not None, "l2": f"per-step Data working set ({data_mb:.0f} MB of Data tensors at {nworld} worlds) exceeds the {l2_mb:.0f} MB L2; no explicit flush" if flush is None else f"Data tensors are {data_mb:.0f} MB (<= {l2_mb:.0f} MB L2): 256 MB scratch buffer written between timed steps",
         "vs_baseline_note": "2,729,192 steps/s is the reference's only published number (benchmarks/README.md:48), hardware unstated",
         "sim_steps_before_timed": sim_steps_before_timed, "ncon_mean": ncon_mean, "nefc_mean": nefc_mean, "solver_niter_mean": niter_mean, "solver_niter_hist_0_1_2_3_4plus": niter_hist, "overflow_worlds": ovf, "overflow_bits_or": hex(ovf_bits), "nan_worlds": nan_worlds,
       },
@@ -478,11 +503,12 @@ def run_ours(args):
       "gpu_launches": launches_per_step * args.steps,
       "kernel_ms": kms,
       "roofline": {"bound": "hbm", "kernel": "k_" + top, "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                   "traffic": traffic, "peak_source": "MEASURED_PEAKS.json hbm_gbs (measured)" if peaks else "fallback 6650 GB/s",
+                   "peak_source": "H100 SXM data sheet, 3.35 TB/s HBM3 (not a measured peak)",
                    "algorithmic_bytes_per_launch": bytes_launch, "step_algorithmic_bytes": step_bytes,
-                   "step_frac": step_bytes / (ms_max / args.steps * 1e-3) / 1e9 / peak, "issue": issue},
+                   "step_frac": step_bytes / (ms_max / args.steps * 1e-3) / 1e9 / peak},
       "cpu_baseline": cpu,
       "clocks": clocks,
+      "device": gpu_info(local),
     }
     print(json.dumps(line))
   if dist is not None:

@@ -1,4 +1,4 @@
-/* mjb200.h -- C ABI of the B200-native batched MuJoCo physics step (libmjb200.so).
+/* mjb200.h -- C ABI of the H100-native (sm_90a) batched MuJoCo physics step (libmjb200.so).
  *
  * Drop-in boundary for the step path of google-deepmind/mujoco_warp.  Every entry point replaces a
  * Python function of the reference's public API (paths relative to /root/reference/mujoco_warp/):

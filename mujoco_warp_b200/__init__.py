@@ -1,4 +1,4 @@
-"""mujoco_warp_b200 -- B200-native (sm_100a) batched MuJoCo physics step behind the mujoco_warp API.
+"""mujoco_warp_b200 -- H100-native (sm_90a) batched MuJoCo physics step behind the mujoco_warp API.
 
 Public surface mirrors /root/reference/mujoco_warp/__init__.py for the step path: put_model, put_data, make_data,
 reset_data, step, forward and the individually callable stages; `mjcf.load` stands in for mujoco's MJCF compiler.

@@ -1,7 +1,7 @@
 """ctypes binding of libmjb200.so (the C-ABI in include/mjb200.h).
 
 The library is built in-tree by `__graft_entry__.build()` / `mujoco_warp_b200.build()` with
-`nvcc -gencode arch=compute_100a,code=sm_100a`.  There is NO fallback: if the shared object is missing
+`nvcc -gencode arch=compute_90a,code=sm_90a`.  There is NO fallback: if the shared object is missing
 or a symbol is absent, importing the step path raises.
 """
 
@@ -16,7 +16,7 @@ _CSRC = os.path.join(_PKG, "csrc")
 LIB_PATH = os.environ.get("MJB_LIB", os.path.join(_PKG, "libmjb200.so"))  # MJB_LIB: A/B-test an alternative build
 HEADER_PATH = os.path.join(os.path.dirname(_PKG), "include", "mjb200.h")
 SOURCES = ["capi.cu", "k_position.cu", "k_collision.cu", "k_collision_mesh.cu", "k_constraint.cu", "k_velocity.cu", "k_solver.cu", "k_integrate.cu", "k_implicit.cu", "k_support.cu", "k_sensor.cu"]
-NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_100a,code=sm_100a", "--extended-lambda", "-Xcompiler", "-fPIC", "-shared"]
+NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a", "--extended-lambda", "-Xcompiler", "-fPIC", "-shared"]
 
 _lib = None
 
@@ -34,7 +34,7 @@ def _stale() -> bool:
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-  """Compile every CUDA source for sm_100a into libmjb200.so (nvcc cross-compiles without a GPU).
+  """Compile every CUDA source for sm_90a into libmjb200.so (nvcc cross-compiles without a GPU).
 
   One object per translation unit, compiled in parallel and only when the source or a header changed, then linked."""
   if not (force or _stale()):
@@ -64,7 +64,7 @@ def build(force: bool = False, verbose: bool = False) -> str:
 
   with ThreadPoolExecutor(max_workers=min(len(SOURCES), os.cpu_count() or 4)) as ex:
     objs = list(ex.map(compile_one, SOURCES))
-  subprocess.check_call([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_PATH, *objs])
+  subprocess.check_call([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB_PATH, *objs])
   return LIB_PATH
 
 
@@ -83,7 +83,7 @@ def lib():
   if _lib is not None:
     return _lib
   if not os.path.exists(LIB_PATH):
-    raise RuntimeError(f"{LIB_PATH} not found: run `python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_100a). There is no CPU fallback for the step path.")
+    raise RuntimeError(f"{LIB_PATH} not found: run `python -c 'import __graft_entry__ as g; g.build()'` (nvcc, sm_90a). There is no CPU fallback for the step path.")
   L = ctypes.CDLL(LIB_PATH)
   vp, cp, ci, cf = ctypes.c_void_p, ctypes.c_char_p, ctypes.c_int, ctypes.c_float
   L.mjb_last_error.restype = cp

@@ -65,7 +65,7 @@ _CONVEX_PAIRS = {
 
 def _require_cuda():
   if not torch.cuda.is_available():
-    raise RuntimeError("mujoco_warp_b200 runs its step path on a CUDA (sm_100a) device only; no CPU fallback exists")
+    raise RuntimeError("mujoco_warp_b200 runs its step path on a CUDA (sm_90a) device only; no CPU fallback exists")
   return torch.device("cuda", torch.cuda.current_device())
 
 

@@ -46,7 +46,7 @@ constexpr size_t kMaxSmem = 227 * 1024;
 extern "C" {
 
 const char* mjb_last_error(void) { return g_err.c_str(); }
-const char* mjb_version(void) { return "mjb200 0.1 (sm_100a)"; }
+const char* mjb_version(void) { return "mjb200 0.1 (sm_90a)"; }
 int mjb_last_launch_count(void) { return g_launches; }
 
 mjbModel* mjb_model_create(void) {
@@ -151,8 +151,8 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
   MJB_DATA_IARRS(X)
 #undef X
   if (d->dev.nv_pad < m->dev.nv) return fail("nv_pad < nv");
-  // nv > 32 solver: Jacobian rows staged in shared memory.  0 (rows are read through L2) measured fastest on B200 -- the smaller
-  // per-world slice lets more worlds share an SM: unitree G1 3.63 -> 4.63 M steps/s, three_humanoids 0.98 -> 1.15 M (48 rows before)
+  // nv > 32 solver: Jacobian rows staged in shared memory.  0 (rows are read through L2) by default: the smaller per-world slice lets
+  // more worlds share an SM
   { const char* e = getenv("MJB_JCAP"); d->dev.jcap = e ? atoi(e) : 0; if (d->dev.jcap < 0) d->dev.jcap = 0; }
   if (check(cudaMalloc(&d->dev.world_conadr, sizeof(int) * (size_t)d->dev.nworld), "cudaMalloc(world_conadr)")) return -1;
   if (check(cudaMalloc(&d->dev.world_ncon, sizeof(int) * (size_t)d->dev.nworld), "cudaMalloc(world_ncon)")) return -1;
@@ -178,8 +178,8 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
     // equality rows read cvel / cdof_dot of the previous step (constraint.py:1085-1117 uses them as they stand when make_constraint
     // runs), which k_velocity overwrites: models with equalities keep the serial chain
     const char* e = getenv("MJB_FORK");
-    // off by default: measured neutral on B200 (humanoid 8192 worlds: 472 -> 475 us) -- both branches are shared-memory bound, so
-    // running them side by side does not raise the number of resident warps; MJB_FORK=1 enables it (bit-identical results, tested)
+    // off by default: both branches are shared-memory bound, so running them side by side does not raise the number of resident
+    // warps; MJB_FORK=1 enables it (bit-identical results, tested)
     d->fork_velocity = (e ? atoi(e) != 0 : false) && m->dev.neq == 0 && d->dev.nworld >= 1024;
   }
   if (m->dev.integrator == INT_RK4 && !d->rk &&

@@ -7,7 +7,7 @@
 // mjb_colliders.cuh; only in the k_collision<8> instantiation, chosen when the model has such geoms),
 // collision_core.py:213-470 (write_contact, contact parameter mixing).
 //
-// B200 design: one warp owns one world.  Lanes test the model's precomputed pair list, survivors are compacted with
+// Design: one warp owns one world.  Lanes test the model's precomputed pair list, survivors are compacted with
 // ballot/popc in pair order, narrowphase runs densely on the compacted list, contacts are staged in shared memory and the
 // world claims ONE contiguous block of the global contact pool with a single atomicAdd (the reference issues one atomic
 // per pair and one per contact).  Within a world the contact order is deterministic (pair order, then contact index);

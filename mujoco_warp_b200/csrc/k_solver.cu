@@ -323,7 +323,7 @@ __device__ __forceinline__ float newton_direction_reg(Ctx& c, int nlist, float g
       }
     }
   }
-#ifdef MJB_CHOL_UNROLLED  // measured slower on B200 (humanoid solver 237 -> 290 us): the straight-line sweep misses the instruction cache
+#ifdef MJB_CHOL_UNROLLED  // off by default: the straight-line sweep misses the instruction cache (see mjb_chol.cuh)
   return chol_solve_rows_unrolled<N>(a, nv, g, c.Lf, lane);
 #else
   c.factored = true;
@@ -850,14 +850,14 @@ static int solver_warps(const ModelDev& m) {
   static int forced = -1;
   if (forced < 0) { const char* e = getenv("MJB_SOLVER_WARPS"); forced = e ? atoi(e) : 0; }
   if (forced == 1 || forced == 2 || forced == 4) return forced;
-  return 1;  // measured on B200: teams of 2 / 4 warps are slower on unitree G1 (3.2 M vs 3.6 M steps/s) and three_humanoids
+  return 1;  // teams of 2 / 4 warps measured slower on unitree G1 and three_humanoids (block barriers per Cholesky column)
 }
 
 // row-capacity classes (see k_solver_classify): small-model path with a staged Jacobian, enough rows and worlds to matter
 static bool solver_uses_classes(const ModelDev& m, const DataDev& d) {
   static int classes = -1;
-  // off by default: measured slower on B200 (humanoid 8192 worlds: solver 237 -> 247 us with every world in the small class, 217 -> 255 us
-  // with a mixed population) -- the extra resident worlds do not speed the solve up, so its time is not set by the number of worlds in
+  // off by default: measured slower for the humanoid, with every world in the small class and with a mixed population -- the extra
+  // resident worlds do not speed the solve up, so its time is not set by the number of worlds in
   // flight the way the position / velocity kernels' is; kept as an experiment knob (MJB_SOLVER_CLASSES=1), parity-tested
   if (classes < 0) { const char* e = getenv("MJB_SOLVER_CLASSES"); classes = e ? atoi(e) : 0; }
   return classes && !solver_big(m) && d.rowcap == 0 && d.njmax >= 32 && d.wn >= 256 && d.sol_list;

@@ -471,8 +471,8 @@ __device__ __forceinline__ float chol_subst_pair(int n, float b, const float* Lc
 
 // The same factor + solve with the column loop fully unrolled: row registers are addressed statically (no rotation), column slots and
 // chunk counts are compile-time, the per-column bookkeeping of the rolled loop (offsets, trip counts, register moves: ~40 of its ~65
-// instructions per column) disappears.  ~1000 instructions for N = 28 instead of ~2300 -- and yet measured SLOWER on B200 (humanoid
-// solver 237 -> 290 us, 150 registers): every warp streams ~16 KB of straight-line code per factorisation through the instruction
+// instructions per column) disappears.  ~1000 instructions for N = 28 instead of ~2300 -- and yet measured SLOWER (150 registers):
+// every warp streams ~16 KB of straight-line code per factorisation through the instruction
 // cache.  Kept behind MJB_CHOL_UNROLLED for reference; the rolled loop above is what ships.  Lc holds colsub_off(N) floats,
 // laid out for the padded size N (rows >= n are identity padding and produce zero multipliers).
 template <int N>

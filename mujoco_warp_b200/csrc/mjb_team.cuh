@@ -106,7 +106,7 @@ struct Stager {
 };
 
 // Launch shape of a team kernel: lanes per world and warps per block, from the per-world shared-memory footprint.
-// Default 8 lanes per world (4 worlds per warp) and two-warp blocks: measured best on B200 for the humanoid (DESIGN.md); models
+// Default 8 lanes per world (4 worlds per warp) and two-warp blocks: measured best on H100 for the humanoid (DESIGN.md); models
 // whose worlds are too large for that fall back to fewer worlds per warp / one-warp blocks.  MJB_LPW_* / MJB_WPB_* override.
 struct TeamShape { int lpw, wpb; size_t warp_bytes, block_bytes; };
 inline TeamShape team_shape(size_t world_words, const char* env_lpw, const char* env_wpb) {

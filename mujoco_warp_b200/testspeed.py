@@ -1,4 +1,4 @@
-"""mjwarp-testspeed compatible benchmark CLI for the B200 step path.
+"""mjwarp-testspeed compatible benchmark CLI for the H100 step path.
 
   python -m mujoco_warp_b200.testspeed <model.xml|model.npz> --nworld 8192 --nconmax 24 --njmax 64 [--nstep 1000]
       [--keyframe 0] [--replay traj.npz] [--function step] [--format human|short|json] [--event_trace]
@@ -102,7 +102,7 @@ def main(argv=None):
     print(f"Rolling out {a.nstep} steps at dt = {timestep:g}...")
 
   center = torch.from_numpy(np.asarray(mjd.ctrl, dtype=np.float32)).cuda()
-  # "JIT" = build/load of the sm_100a library + CUDA-graph capture of fn(m, d)
+  # "JIT" = build/load of the sm_90a library + CUDA-graph capture of fn(m, d)
   t0 = time.perf_counter()
   stream = torch.cuda.Stream()
   with torch.cuda.stream(stream):

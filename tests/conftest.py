@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-  config.addinivalue_line("markers", "gpu: test needs a CUDA (B200) device")
+  config.addinivalue_line("markers", "gpu: test needs a CUDA (H100) device")
 
 
 @pytest.fixture(scope="session")

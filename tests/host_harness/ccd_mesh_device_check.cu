@@ -1,4 +1,4 @@
-// Test-only: the CCD_MESH build of mjb_ccd.cuh must compile as device code for sm_100a (tests/test_device_ccd_mesh_on_host.py runs nvcc -c on
+// Test-only: the CCD_MESH build of mjb_ccd.cuh must compile as device code for sm_90a (tests/test_device_ccd_mesh_on_host.py runs nvcc -c on
 // this file).  One thread per pair, geoms given by descriptor -- the shape the collision kernel's convex pass will call it in.
 #define CCD_MESH 1
 #include "../../mujoco_warp_b200/csrc/mjb_ccd.cuh"

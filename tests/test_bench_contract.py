@@ -1,6 +1,6 @@
 """bench.py's reference arm (`--impl reference`: the CPU restatement timed on the host cores) runs without a GPU, so its JSON line --
 the part of the benchmark contract the driver parses for both arms -- is checked here; the GPU arm prints the same keys plus `roofline`,
-`kernel_ms` and `clocks` (profiles/r02_bench.json is a committed example)."""
+`kernel_ms`, `clocks` and `device` (profiles/bench_h100.json is a committed example)."""
 
 import json
 import os
@@ -37,8 +37,8 @@ def test_reference_arm_other_ranks_exit_quietly():
 
 
 def test_committed_gpu_line_has_the_contract_keys():
-  d = json.load(open(os.path.join(ROOT, "profiles", "r02_bench.json")))
-  for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline", "dtype", "data", "config", "e2e", "gpu_launches", "roofline", "cpu_baseline", "clocks"):
+  d = json.load(open(os.path.join(ROOT, "profiles", "bench_h100.json")))
+  for k in ("metric", "value", "unit", "n_gpus", "steps", "warmup", "ms_per_step", "higher_is_better", "scaling", "vs_baseline", "dtype", "data", "config", "e2e", "gpu_launches", "roofline", "cpu_baseline", "clocks", "device"):
     assert k in d, k
   r = d["roofline"]
   assert r["bound"] == "hbm" and abs(r["frac"] - r["achieved"] / r["peak"]) < 1e-9 and r["unit"] == "GB/s"

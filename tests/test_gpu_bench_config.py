@@ -4,7 +4,8 @@ and rows are cut at njmax (the state bench.py times).  Every 20 steps the fp32 b
 state (teacher forcing: a free-running comparison of two fp32 implementations of a contact-rich system diverges chaotically after a
 few dozen steps, which says nothing about either) and must agree per world: exact nefc / ne / nf / nl, exact contact count,
 exact overflow bits raised by the step, state within the fp32 band.  Contact make / break decisions sit at |dist - margin| ~ 1e-7
-boundaries, so a handful of worlds per checkpoint may legitimately differ by one contact; the budget is 0.25 % of the worlds.
+boundaries, so a handful of worlds per checkpoint may legitimately differ by one contact: worlds with a contact within 1e-6 of its margin
+on either side may differ in up to 0.1 % of the worlds (at least 4), any other difference in up to 0.25 %.
 
 Also covers the world-split pipeline (MJB_SPLIT = 1, 2, 3 on internal streams, plain launches and graph replay) on the same
 state: per-world results must be bit-identical whatever the split (ADVICE r1: the default split was never tested)."""
@@ -21,6 +22,7 @@ from tests import util
 pytestmark = pytest.mark.gpu
 
 NWORLD, NCONMAX, NJMAX = 8192, 24, 64
+EDGE = 1e-6  # |dist - margin| of a contact whose make / break decision is a matter of fp32 rounding (a few ulp of a body position)
 
 
 def _bench_state(mjw, mjm, m, nworld):
@@ -55,6 +57,10 @@ def _lockstep(mjw, NWORLD, njmax, nsteps):
   o = util.make_oracle(mjm, NWORLD, NCONMAX, njmax, dtype=np.float32)
   stream = torch.cuda.Stream()
   budget = max(2, NWORLD // 400)  # 0.25 % of the worlds per checkpoint (observed: up to 10 of 8192 while the humanoid is falling, step ~100)
+  # worlds whose difference comes with a contact at its margin (below).  Observed on an H100 over the 20 checkpoints: at most 6 of 8192
+  # worlds (step 99; 1-4 at ten others, none at the remaining nine) and 3 of 1024 with njmax 40 (steps 99 and 299), while the other
+  # differences stayed at 0 of 8192 and at most 1 of 1024
+  edge_budget = max(4, NWORLD // 1000)
   seen_overflow, max_nefc = 0, 0
   with torch.cuda.stream(stream):
     mjw.step(m, d)  # warm-up launch configures shared memory sizes before capture
@@ -79,13 +85,19 @@ def _lockstep(mjw, NWORLD, njmax, nsteps):
       o.set_state(**state)
       o.d["overflow"][:] = 0
       o.step()
-      for f in ("nefc", "ne", "nf", "nl"):
-        bad = int((getattr(d, f).cpu().numpy() != o.d[f]).sum())
-        assert bad <= budget, f"step {i}: {f} differs in {bad} worlds (budget {budget})"
-      wid = d.contact.worldid[: int(d.nacon.cpu()[0])].cpu().numpy()
+      nacon = int(d.nacon.cpu()[0])
+      wid = d.contact.worldid[:nacon].cpu().numpy()
       ncon_gpu = np.bincount(wid, minlength=NWORLD)
-      bad = int((ncon_gpu != o.d["ncon"]).sum())
-      assert bad <= budget, f"step {i}: contact count differs in {bad} worlds (budget {budget})"
+      # worlds with a contact within fp32 rounding of its margin on either side count against `edge_budget`, all others against `budget`
+      edge = np.zeros(NWORLD, dtype=bool)
+      np.logical_or.at(edge, wid, (d.contact.dist[:nacon] - d.contact.includemargin[:nacon]).abs().cpu().numpy() < EDGE)
+      live = np.arange(o.d["con_dist"].shape[1])[None, :] < o.d["ncon"][:, None]
+      edge |= (live & (np.abs(o.d["con_dist"] - o.d["con_includemargin"]) < EDGE)).any(axis=1)
+      for f, gpu in (("nefc", d.nefc), ("ne", d.ne), ("nf", d.nf), ("nl", d.nl), ("contact count", ncon_gpu)):
+        differ = (gpu.cpu().numpy() if isinstance(gpu, torch.Tensor) else gpu) != o.d["ncon" if f == "contact count" else f]
+        bad, at_edge = int((differ & ~edge).sum()), int((differ & edge).sum())
+        assert bad <= budget, f"step {i}: {f} differs in {bad} worlds without a contact at its margin (budget {budget})"
+        assert at_edge <= edge_budget, f"step {i}: {f} differs in {at_edge} worlds with a contact at its margin (budget {edge_budget})"
       same = (d.nefc.cpu().numpy() == o.d["nefc"]) & (ncon_gpu == o.d["ncon"])
       # overflow bits of this step (njmax truncation -> NEFC ...); the line-search budget bit may differ at rounding level
       mask = ~int(mjw.OverflowType.LS_ITERATIONS)

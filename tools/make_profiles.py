@@ -41,7 +41,7 @@ cols = ["gpu__time_duration.sum", "smsp__inst_executed.sum", "smsp__thread_inst_
 st = [h for h in hdr if "smsp__average_warps_issue_stalled" in h and h.endswith("per_issue_active.ratio")]
 traffic, winst = {}, {}
 with open(os.path.join(P, f"{R}_kernels.md"), "w") as f:
-  f.write(f"# ncu --set full --clock-control none, {R} kernels (humanoid, 8192 worlds, 1xB200, MJB_SPLIT=1 so each kernel covers all worlds; step 120 from the squat keyframe, the middle of the bench window)\n\n")
+  f.write(f"# ncu --set full --clock-control none, {R} kernels (humanoid, 8192 worlds, one GPU, MJB_SPLIT=1 so each kernel covers all worlds; step 120 from the squat keyframe, the middle of the bench window)\n\n")
   f.write("Units as ncu reports them (time us, DRAM Mbyte, shared memory Kbyte/block).  `thread_inst / inst` = average active lanes per warp instruction.\n\n")
   f.write("| kernel | " + " | ".join(c.split("__")[-1].replace(".sum", "").replace(".avg.pct_of_peak_sustained_", " % ").replace(".ratio", "")[:34] for c in cols) + " | top stalls (warps per issue-active cycle) |\n")
   f.write("|---|" + "---|" * (len(cols) + 1) + "\n")
@@ -71,7 +71,7 @@ for line in sass.splitlines():
       counts.setdefault(fn, collections.Counter())[mn] += 1
 with open(os.path.join(P, f"{R}_sass_tma.md"), "w") as f:
   f.write("# Bulk-async (1-D TMA) staging in the shipped SASS (`cuobjdump -sass mujoco_warp_b200/libmjb200.so`)\n\n")
-  f.write("`cp.async.bulk` appears as `UBLKCP` (global -> shared with `.S.G`, shared -> global with `.G.S`), the mbarrier transaction count as `SYNCS.ARRIVE.TRANS64`, the wait as\n`SYNCS.PHASECHK.TRANS64.TRYWAIT`, the generic -> async proxy fence as `FENCE.VIEW.ASYNC` (B200_PROFILING.md, B300_MICROARCH.md).  Instruction counts per kernel:\n\n| kernel | UBLKCP | SYNCS.ARRIVE.TRANS64 | SYNCS.PHASECHK | FENCE.VIEW.ASYNC |\n|---|---|---|---|---|\n")
+  f.write("`cp.async.bulk` appears as `UBLKCP` (global -> shared with `.S.G`, shared -> global with `.G.S`), the mbarrier transaction count as `SYNCS.ARRIVE.TRANS64`, the wait as\n`SYNCS.PHASECHK.TRANS64.TRYWAIT`, the generic -> async proxy fence as `FENCE.VIEW.ASYNC`.  Instruction counts per kernel:\n\n| kernel | UBLKCP | SYNCS.ARRIVE.TRANS64 | SYNCS.PHASECHK | FENCE.VIEW.ASYNC |\n|---|---|---|---|---|\n")
   for k, c in counts.items():
     if c["UBLKCP"]:
       f.write(f"| `{k[:110]}` | {c['UBLKCP']} | {c['SYNCS.ARRIVE.TRANS64']} | {c['SYNCS.PHASECHK']} | {c['FENCE.VIEW.ASYNC']} |\n")
