@@ -112,6 +112,11 @@ int mjb_ctrl_noise(const mjbModel* m, mjbData* d, const float* ctrl_center, int 
  * velocity, solver, integrate), synchronises, and writes the 6 durations in ms to ms_out (host pointer). */
 int mjb_step_profile(const mjbModel* m, mjbData* d, void* stream, float* ms_out);
 
+/* worlds per SM that are resident at once (cudaOccupancyMaxActiveBlocksPerMultiprocessor times worlds per block) in the launch
+ * shape k_position / k_velocity take for all of d's worlds.  Both kernels are latency bound: they finish in
+ * ceil(nworld / (SMs x worlds per SM)) rounds of one world's dependent chain. */
+int mjb_team_residency(const mjbModel* m, const mjbData* d, int* position_worlds, int* velocity_worlds);
+
 /* number of kernels the last mjb_* pipeline call launched (for bench.py's gpu_launches) */
 int mjb_last_launch_count(void);
 const char* mjb_last_error(void);

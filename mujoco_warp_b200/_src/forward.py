@@ -273,3 +273,15 @@ def step_profile(m: Model, d: Data):
   stream = torch.cuda.current_stream().cuda_stream
   _lib.check(_lib.lib().mjb_step_profile(m._handle, d._handle, stream, out))
   return dict(zip(KERNEL_NAMES, [float(x) for x in out]))
+
+
+def team_residency(m: Model, d: Data):
+  """Worlds per SM resident at once in the launch shape of k_position / k_velocity for all of d's worlds (occupancy API);
+  returns {"position": n, "velocity": n}."""
+  import ctypes
+
+  f = _lib.lib().mjb_team_residency
+  f.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]
+  pos, vel = ctypes.c_int(), ctypes.c_int()
+  _lib.check(f(m._handle, d._handle, ctypes.byref(pos), ctypes.byref(vel)))
+  return {"position": pos.value, "velocity": vel.value}

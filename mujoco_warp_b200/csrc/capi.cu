@@ -184,8 +184,8 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
   }
   if (m->dev.integrator == INT_RK4 && !d->rk &&
       check(cudaMalloc(&d->rk, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nq + 3 * m->dev.nv + 2 * m->dev.na + 1)), "cudaMalloc(rk)")) return -1;
-  d->smem[0] = smem_position(m->dev); d->smem[1] = smem_collision(m->dev, d->dev); d->smem[2] = smem_constraint(m->dev, d->dev);
-  d->smem[3] = smem_velocity(m->dev); d->smem[4] = smem_solver(m->dev, d->dev); d->smem[5] = smem_integrate(m->dev);
+  d->smem[0] = smem_position(m->dev, d->dev); d->smem[1] = smem_collision(m->dev, d->dev); d->smem[2] = smem_constraint(m->dev, d->dev);
+  d->smem[3] = smem_velocity(m->dev, d->dev); d->smem[4] = smem_solver(m->dev, d->dev); d->smem[5] = smem_integrate(m->dev);
   static const char* names[6] = {"position", "collision", "constraint", "velocity", "solver", "integrate"};
   for (int i = 0; i < 6; i++)
     if (d->smem[i] > kMaxSmem) {
@@ -359,6 +359,13 @@ int mjb_step_profile(const mjbModel* m, mjbData* d, void* stream, float* ms_out)
   if (check(cudaEventSynchronize(ev[6]), "cudaEventSynchronize")) return -1;
   for (int i = 0; i < 6; i++) cudaEventElapsedTime(&ms_out[i], ev[i], ev[i + 1]);
   for (int i = 0; i < 7; i++) cudaEventDestroy(ev[i]);
+  return 0;
+}
+int mjb_team_residency(const mjbModel* m, const mjbData* d, int* position_worlds, int* velocity_worlds) {
+  if (!m || !d || !m->finalized || !d->finalized) return fail("model/data not finalized");
+  if (!position_worlds || !velocity_worlds) return fail("mjb_team_residency: null output");
+  if (check(resident_worlds_position(m->dev, d->dev, position_worlds), "resident_worlds_position")) return -1;
+  if (check(resident_worlds_velocity(m->dev, d->dev, velocity_worlds), "resident_worlds_velocity")) return -1;
   return 0;
 }
 int mjb_ctrl_noise(const mjbModel* m, mjbData* d, const float* ctrl_center, int step, float noise_std, float noise_rate, void* stream) {

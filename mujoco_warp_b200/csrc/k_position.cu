@@ -16,33 +16,31 @@
 namespace {
 
 struct PosLayout {
-  int qpos, xpos, xquat, xipos, xanchor, xaxis, scom, cinert, cdof, buf, arena, a_gxmat, total;
+  int qpos, xpos, xquat, xipos, xanchor, xaxis, scom, cinert, cdof, buf, arena, gxpos, gxmat, M, total;
 };
 
 // Per-world words of shared memory.  Only what later phases read stays resident (body poses, joint anchors / axes, subtree
-// com, cinert -> crb in place, cdof); pure outputs (xmat, ximat, geom poses, M) pass one after the other through one arena
-// that is reused once the bulk store that read it has drained; qpos sits in the arena until the tree pass is done, and the
-// crb * cdof scratch takes the place of the body / joint poses once those have left.  3.8 KB per humanoid world: an SM holds
-// its 55 worlds at once.  That is what the kernel time hangs on -- it is latency bound (ncu: one instruction issued per ~13
-// cycles per warp, long-scoreboard stalls on dependent table lookups), so time ~ rounds of resident worlds x per-warp chain.
+// com, cinert -> crb in place, cdof); pure outputs pass through space whose bulk store has drained:
+//  - the arena holds qpos until the tree pass and the transmission are done, then xmat, then ximat;
+//  - geom_xpos and geom_xmat are built from xipos on: xipos, xanchor, xaxis, subtree_com and the arena have all been stored by then;
+//  - the crb * cdof scratch and then M are built from xpos on, once the body poses have left.
+// 3.3 KB per humanoid world, so that an SM holds 64 worlds at once and 8192 worlds fit on 132 SMs in one round.  That is what
+// the kernel time hangs on -- it is latency bound (ncu: one instruction issued per ~13 cycles per warp, long-scoreboard stalls
+// on dependent table lookups), so time ~ rounds of resident worlds x per-warp chain (DESIGN.md §3).
 __host__ __device__ inline int pad4(int n) { return (n + 3) & ~3; }
 __host__ __device__ inline PosLayout pos_layout(const ModelDev& m) {
   PosLayout L;
   int o = 0;
   auto take = [&](int n) { int r = o; o += pad4(n); return r; };  // padded: a field's group block [G][n] starts 16 B aligned
   L.xpos = take(3 * m.nbody); L.xquat = take(4 * m.nbody); L.xipos = take(3 * m.nbody);
-  L.xanchor = take(3 * m.njnt); L.xaxis = take(3 * m.njnt);
-  L.buf = L.xpos;
-  if (o < pad4(6 * m.nv)) o = pad4(6 * m.nv);
-  L.scom = take(3 * m.nbody); L.cinert = take(10 * m.nbody); L.cdof = take(6 * m.nv);
-  // arena uses, in time order: qpos (tree pass, transmission), xmat, ximat, [geom_xpos | geom_xmat], M
-  L.a_gxmat = pad4(3 * m.ngeom);
-  int a = pad4(9 * m.nbody);
-  if (L.a_gxmat + pad4(9 * m.ngeom) > a) a = L.a_gxmat + pad4(9 * m.ngeom);
-  if (pad4(m.nC) > a) a = pad4(m.nC);
-  if (pad4(m.nq) > a) a = pad4(m.nq);
-  L.arena = take(a);
+  L.xanchor = take(3 * m.njnt); L.xaxis = take(3 * m.njnt); L.scom = take(3 * m.nbody);
+  L.arena = take(pad4(m.nq) > pad4(9 * m.nbody) ? m.nq : 9 * m.nbody);
   L.qpos = L.arena;
+  L.gxpos = L.xipos; L.gxmat = L.gxpos + pad4(3 * m.ngeom);
+  L.buf = L.xpos; L.M = L.buf + pad4(6 * m.nv);
+  if (o < L.gxmat + pad4(9 * m.ngeom)) o = L.gxmat + pad4(9 * m.ngeom);
+  if (o < L.M + pad4(m.nC)) o = L.M + pad4(m.nC);
+  L.cinert = take(10 * m.nbody); L.cdof = take(6 * m.nv);
   L.total = o;
   return L;
 }
@@ -65,15 +63,14 @@ k_position(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
   Stager st;
   st.init(reinterpret_cast<uint64_t*>(S + (size_t)L.total * G), lane);
   const int nb = m.nbody, nj = m.njnt, ng = m.ngeom, nv = m.nv;
-  // block (all G worlds) and this team's row of a resident field / of an arena slot at per-world offset `off`
+  // block (all G worlds) and this team's row of a field
 #define BLK(f) (S + (size_t)L.f * G)
-#define ABLK(off) (S + (size_t)(L.arena + (off)) * G)
 #define ROW(blk, n) ((blk) + (size_t)g * (n))
   float *qpos = ROW(BLK(qpos), m.nq), *xpos = ROW(BLK(xpos), 3 * nb), *xquat = ROW(BLK(xquat), 4 * nb), *xipos = ROW(BLK(xipos), 3 * nb),
         *xanchor = ROW(BLK(xanchor), 3 * nj), *xaxis = ROW(BLK(xaxis), 3 * nj), *scom = ROW(BLK(scom), 3 * nb), *cinert = ROW(BLK(cinert), 10 * nb),
         *cdof = ROW(BLK(cdof), 6 * nv);
-  float *xmat = ROW(ABLK(0), 9 * nb), *ximat = ROW(ABLK(0), 9 * nb), *gxpos = ROW(ABLK(0), 3 * ng), *gxmat = ROW(ABLK(L.a_gxmat), 9 * ng),
-        *buf = ROW(BLK(buf), 6 * nv), *Ms = ROW(ABLK(0), m.nC);
+  float *xmat = ROW(BLK(arena), 9 * nb), *ximat = ROW(BLK(arena), 9 * nb), *gxpos = ROW(BLK(gxpos), 3 * ng), *gxmat = ROW(BLK(gxmat), 9 * ng),
+        *buf = ROW(BLK(buf), 6 * nv), *Ms = ROW(BLK(M), m.nC);
   float* crb = cinert;  // accumulated in place once cinert has been stored
   // the G worlds' rows of a Data field are one contiguous block in global memory
   const size_t wg = (size_t)T.wg0;
@@ -195,7 +192,7 @@ k_position(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
       for (int k = 0; k < 9; k++) d.site_xmat[(wb * m.nsite + s) * 9 + k] = mat[k];
     }
     st.store_fence();
-    GSTORE(xpos, BLK(xpos), 3 * nb); GSTORE(xquat, BLK(xquat), 4 * nb); GSTORE(xmat, ABLK(0), 9 * nb); GSTORE(xipos, BLK(xipos), 3 * nb);
+    GSTORE(xpos, BLK(xpos), 3 * nb); GSTORE(xquat, BLK(xquat), 4 * nb); GSTORE(xmat, BLK(arena), 9 * nb); GSTORE(xipos, BLK(xipos), 3 * nb);
     GSTORE(xanchor, BLK(xanchor), 3 * nj); GSTORE(xaxis, BLK(xaxis), 3 * nj);
     st.store_commit();
     if (!com) {  // kinematics alone: the inertial frames follow xmat through the arena (otherwise the cinert loop below produces them)
@@ -203,7 +200,7 @@ k_position(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
 #pragma unroll 2
       for (int b = sub; b < nb; b += LPW) quat_to_mat(qmul(ldq(xquat + 4 * b), ldq(m.body_iquat + 4 * b)), ximat + 9 * b);
       st.store_fence();
-      GSTORE(ximat, ABLK(0), 9 * nb);
+      GSTORE(ximat, BLK(arena), 9 * nb);
       st.store_commit();
     }
   }
@@ -278,7 +275,7 @@ k_position(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
     }
     st.store_fence();
     GSTORE(subtree_com, BLK(scom), 3 * nb); GSTORE(cinert, BLK(cinert), 10 * nb); GSTORE(cdof, BLK(cdof), 6 * nv);
-    if (kin) GSTORE(ximat, ABLK(0), 9 * nb);
+    if (kin) GSTORE(ximat, BLK(arena), 9 * nb);
     st.store_commit();
   }
   __syncwarp();
@@ -337,7 +334,7 @@ k_position(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
   }
 
 
-  // ------------------------------------------------------------------ kinematics: geom poses (through the arena, once xmat / ximat have left)
+  // ------------------------------------------------------------------ kinematics: geom poses (from xipos on, once xipos .. ximat have been stored)
   if (kin) {
     st.store_wait_read();
 #pragma unroll 2
@@ -353,13 +350,13 @@ k_position(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
       }
     }
     st.store_fence();
-    GSTORE(geom_xpos, ABLK(0), 3 * ng); GSTORE(geom_xmat, ABLK(L.a_gxmat), 9 * ng);
+    GSTORE(geom_xpos, BLK(gxpos), 3 * ng); GSTORE(geom_xmat, BLK(gxmat), 9 * ng);
     st.store_commit();
   }
 
   // ------------------------------------------------------------------ crb + M (smooth.py:1029-1098)
   if (crbm) {
-    st.store_wait_read();  // cinert has been stored: crb accumulates in place; the arena and the pose fields (-> buf) are free
+    st.store_wait_read();  // cinert has been stored: crb accumulates in place; the geom poses have been stored: xpos on (-> buf, M) is free
 #pragma unroll 1
     for (int l = m.nlevel - 2; l >= 1; l--) {
 #pragma unroll 1
@@ -390,39 +387,53 @@ k_position(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
       Ms[e] = v;
     }
     st.store_fence();
-    GSTORE(crb, BLK(cinert), 10 * nb); GSTORE(M, ABLK(0), m.nC);
+    GSTORE(crb, BLK(cinert), 10 * nb); GSTORE(M, BLK(M), m.nC);
     st.store_commit();
   }
   st.store_wait_read();  // shared memory must outlive the bulk stores that read it
 #undef GLOAD
 #undef GSTORE
 #undef BLK
-#undef ABLK
 #undef ROW
 }
 
 }  // namespace
 
-static TeamShape pos_shape(const ModelDev& m) {
-  TeamShape t = team_shape((size_t)pos_layout(m).total, "MJB_LPW_POS", "MJB_WPB_POS");
+static void (*pos_kernel(const ModelDev& m, int lpw))(ModelDev, DataDev, int) {
+  return m.batched ? k_position<32, true> : lpw == 4 ? k_position<4, false> : lpw == 8 ? k_position<8, false> : lpw == 16 ? k_position<16, false> : k_position<32, false>;
+}
+
+static TeamShape pos_shape(const ModelDev& m, const DataDev& d) {
+  TeamShape t = team_shape((size_t)pos_layout(m).total, d.wn, "MJB_LPW_POS", "MJB_WPB_POS", [&](int lpw) { return kernel_regs(pos_kernel(m, lpw)); });
   if (m.batched && t.lpw != 32) { t = team_shape_fixed((size_t)pos_layout(m).total, 32, 2); }
   return t;
 }
-size_t smem_position(const ModelDev& m) { return pos_shape(m).block_bytes; }
+size_t smem_position(const ModelDev& m, const DataDev& d) { return pos_shape(m, d).block_bytes; }
+
+// the kernel instance for the launch shape, configured on its first use
+static cudaError_t pos_configured(const ModelDev& m, const TeamShape& t, void (**kern)(ModelDev, DataDev, int)) {
+  static TeamConfig configured[5];
+  const int lpw = t.lpw, ki = m.batched ? 4 : lpw == 4 ? 0 : lpw == 8 ? 1 : lpw == 16 ? 2 : 3;
+  *kern = pos_kernel(m, lpw);
+  return team_configure(*kern, t.block_bytes, &configured[ki]);
+}
 
 cudaError_t launch_position(const ModelDev& m, const DataDev& d, int mask, cudaStream_t s) {
-  const TeamShape t = pos_shape(m);
-  const size_t smem = t.block_bytes;
-  const int lpw = t.lpw, G = 32 / lpw, wpb = t.wpb;
-  void (*kern)(ModelDev, DataDev, int) = m.batched ? k_position<32, true> : lpw == 4 ? k_position<4, false> : lpw == 8 ? k_position<8, false> : lpw == 16 ? k_position<16, false> : k_position<32, false>;
-  static size_t configured[5] = {0, 0, 0, 0, 0};
-  const int ki = m.batched ? 4 : lpw == 4 ? 0 : lpw == 8 ? 1 : lpw == 16 ? 2 : 3;
-  if (smem > 48 * 1024 && smem > configured[ki]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    configured[ki] = smem;
-  }
-  const int ngroups = (d.wn + G - 1) / G, grid = (ngroups + wpb - 1) / wpb;
-  kern<<<grid, 32 * wpb, smem, s>>>(m, d, mask);
+  const TeamShape t = pos_shape(m, d);
+  void (*kern)(ModelDev, DataDev, int);
+  cudaError_t e = pos_configured(m, t, &kern);
+  if (e != cudaSuccess) return e;
+  const int G = 32 / t.lpw, ngroups = (d.wn + G - 1) / G, grid = (ngroups + t.wpb - 1) / t.wpb;
+  kern<<<grid, 32 * t.wpb, t.block_bytes, s>>>(m, d, mask);
   return cudaGetLastError();
+}
+
+cudaError_t resident_worlds_position(const ModelDev& m, const DataDev& d, int* worlds) {
+  const TeamShape t = pos_shape(m, d);
+  void (*kern)(ModelDev, DataDev, int);
+  int blocks = 0;
+  cudaError_t e = pos_configured(m, t, &kern);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, 32 * t.wpb, t.block_bytes);
+  *worlds = blocks * t.wpb * (32 / t.lpw);
+  return e;
 }

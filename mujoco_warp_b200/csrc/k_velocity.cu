@@ -19,23 +19,33 @@
 namespace {
 
 struct VelLayout { int qvel, cdof, cinert, cvel, cdofdot, cacc, cfrc, qpas, qbias, qact, qsm, qld, x, af, total; };
-// Per-world words of shared memory (3.9 KB for the humanoid, so that an SM's 55 worlds are resident together: the kernel is
-// latency bound).  The n x n factor (Data.qLD layout) is built where the tree-pass fields (cdof .. cfrc_int) lived, once the
-// bulk stores that read them have drained; M is scattered into it straight from global memory.
+// Per-world words of shared memory, sized by what is live in each phase: 3.1 KB for the humanoid, so that an SM holds 64 worlds
+// at once and 8192 worlds fit on 132 SMs in one round (the kernel is latency bound, DESIGN.md §3).  qfrc_passive and qfrc_bias
+// stay live until qfrc_smooth is formed and sit outside the region below: qfrc_smooth is formed in place in qfrc_passive's slot
+// (qfrc_passive goes straight to global memory, so no bulk store reads that slot), and the solve's right-hand side / solution
+// takes qfrc_bias's slot once its bulk store has drained.  The region holds, in turn:
+//  - the tree-pass fields; cfrc_int takes cdof_dot's slot (sized for both) once the cacc pass has read it and its bulk store has
+//    drained;
+//  - the actuation fields (qfrc_actuator, actuator forces) in the slots of cinert and qvel, both dead after rne and never the
+//    source of a bulk store (or past the tree-pass fields when they do not fit there);
+//  - the n x n factor (Data.qLD layout), once the bulk stores that read the region have drained; M is scattered into it straight
+//    from global memory.  cdof stays intact until then: the applied-wrench term of qfrc_smooth reads it.
 __host__ __device__ inline VelLayout vel_layout(const ModelDev& m) {
   VelLayout L;
   int o = 0;
-  auto take = [&](int n) { int r = o; o += (n + 3) & ~3; return r; };  // padded: a field's group block [G][n] starts 16 B aligned
-  L.qvel = take(m.nv);
+  auto pad = [](int n) { return (n + 3) & ~3; };  // padded: a field's group block [G][n] starts 16 B aligned
+  auto take = [&](int n) { int r = o; o += pad(n); return r; };
+  L.qpas = take(m.nv); L.qbias = take(m.nv);
+  L.qsm = L.qpas; L.x = L.qbias;
   const int a0 = o;
-  L.cdof = take(6 * m.nv); L.cinert = take(10 * m.nbody); L.cvel = take(6 * m.nbody);
-  L.cdofdot = take(6 * m.nv); L.cacc = take(6 * m.nbody); L.cfrc = take(6 * m.nbody);
+  L.cdof = take(6 * m.nv); L.cinert = take(10 * m.nbody); L.qvel = take(m.nv);
+  // cdof_dot's slot also holds cfrc_int later, so it is sized for the larger of the two (models with more bodies than dofs / 6)
+  L.cvel = take(6 * m.nbody); L.cdofdot = take(6 * (m.nv > m.nbody ? m.nv : m.nbody)); L.cacc = take(6 * m.nbody);
+  L.cfrc = L.cdofdot;
+  if (pad(m.nv) + pad(m.nu) <= L.cvel - L.cinert) { L.qact = L.cinert; L.af = L.cinert + pad(m.nv); }
+  else { L.qact = take(m.nv); L.af = take(m.nu); }
   L.qld = a0;
-  if (o - a0 < ((m.qld_total + 3) & ~3)) o = a0 + ((m.qld_total + 3) & ~3);
-  L.qpas = take(m.nv); L.qbias = take(m.nv); L.qact = take(m.nv); L.qsm = take(m.nv);
-  // the solve's right-hand side / solution takes qfrc_passive's slot once qfrc_smooth has been formed (qfrc_passive is written
-  // straight to global memory); actuator forces live in their own small slot
-  L.x = L.qpas; L.af = take(m.nu);
+  if (o - a0 < pad(m.qld_total)) o = a0 + pad(m.qld_total);
   L.total = o;
   return L;
 }
@@ -291,6 +301,7 @@ k_velocity(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
       }
       __syncwarp();
     }
+    st.store_wait_read();  // cfrc_int takes cdof_dot's slot: the bulk store of cdof_dot must have read it
 #pragma unroll 2
     for (int b = sub; b < nb; b += LPW) {
       float f[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
@@ -442,7 +453,9 @@ k_velocity(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
     }
     // per-tree dense Cholesky of M in the qLD layout (upper factor U, row-major, zeros below), qacc_smooth = M^-1 qfrc_smooth
     const bool acc = mask & STG_ACCELERATION;
-    st.store_wait_read();  // the factor is built where cdof .. cfrc_int lived: their bulk stores must have read them
+    // the factor is built where cdof .. cfrc_int and the actuation fields lived, and the solve vector takes qfrc_bias's slot: the
+    // bulk stores that read them must have drained
+    st.store_wait_read();
 #pragma unroll 1
     for (int i = sub; i < m.qld_total; i += LPW) qld[i] = 0.f;
     if (acc)
@@ -478,32 +491,48 @@ k_velocity(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
 
 }  // namespace
 
-static TeamShape vel_shape(const ModelDev& m) {
-  TeamShape t = team_shape((size_t)vel_layout(m).total, "MJB_LPW_VEL", "MJB_WPB_VEL");
-  if (m.batched && t.lpw != 32) t = team_shape_fixed((size_t)vel_layout(m).total, 32, 2);
-  return t;
-}
-size_t smem_velocity(const ModelDev& m) { return vel_shape(m).block_bytes; }
-
 template <bool PEXT>
 static void (*vel_kernel(int lpw, bool bat))(ModelDev, DataDev, int) {
   if (bat) return k_velocity<PEXT, 32, true>;
   return lpw == 4 ? k_velocity<PEXT, 4, false> : lpw == 8 ? k_velocity<PEXT, 8, false> : lpw == 16 ? k_velocity<PEXT, 16, false> : k_velocity<PEXT, 32, false>;
 }
+// has_gravcomp also flags free / ball joint springs (io.py put_model); tendons live in the same instantiation
+static bool vel_ext(const ModelDev& m) { return m.has_gravcomp || m.ntendon > 0; }
+static void (*vel_kernel(const ModelDev& m, int lpw))(ModelDev, DataDev, int) {
+  return vel_ext(m) ? vel_kernel<true>(lpw, m.batched) : vel_kernel<false>(lpw, m.batched);
+}
+
+static TeamShape vel_shape(const ModelDev& m, const DataDev& d) {
+  TeamShape t = team_shape((size_t)vel_layout(m).total, d.wn, "MJB_LPW_VEL", "MJB_WPB_VEL", [&](int lpw) { return kernel_regs(vel_kernel(m, lpw)); });
+  if (m.batched && t.lpw != 32) t = team_shape_fixed((size_t)vel_layout(m).total, 32, 2);
+  return t;
+}
+size_t smem_velocity(const ModelDev& m, const DataDev& d) { return vel_shape(m, d).block_bytes; }
+
+// the kernel instance for the launch shape, configured on its first use
+static cudaError_t vel_configured(const ModelDev& m, const TeamShape& t, void (**kern)(ModelDev, DataDev, int)) {
+  static TeamConfig configured[2][5];
+  const int ext = vel_ext(m) ? 1 : 0, ki = m.batched ? 4 : t.lpw == 4 ? 0 : t.lpw == 8 ? 1 : t.lpw == 16 ? 2 : 3;
+  *kern = vel_kernel(m, t.lpw);
+  return team_configure(*kern, t.block_bytes, &configured[ext][ki]);
+}
 
 cudaError_t launch_velocity(const ModelDev& m, const DataDev& d, int mask, cudaStream_t s) {
-  const TeamShape t = vel_shape(m);
-  const size_t smem = t.block_bytes;
-  static size_t configured[2][5] = {{0, 0, 0, 0, 0}, {0, 0, 0, 0, 0}};
-  const int ext = (m.has_gravcomp || m.ntendon > 0) ? 1 : 0;  // has_gravcomp also flags free / ball joint springs (io.py put_model); tendons live in the same instantiation
-  const int lpw = t.lpw, G = 32 / lpw, wpb = t.wpb, ki = m.batched ? 4 : lpw == 4 ? 0 : lpw == 8 ? 1 : lpw == 16 ? 2 : 3;
-  void (*kern)(ModelDev, DataDev, int) = ext ? vel_kernel<true>(lpw, m.batched) : vel_kernel<false>(lpw, m.batched);
-  if (smem > 48 * 1024 && smem > configured[ext][ki]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    configured[ext][ki] = smem;
-  }
-  const int ngroups = (d.wn + G - 1) / G, grid = (ngroups + wpb - 1) / wpb;
-  kern<<<grid, 32 * wpb, smem, s>>>(m, d, mask);
+  const TeamShape t = vel_shape(m, d);
+  void (*kern)(ModelDev, DataDev, int);
+  cudaError_t e = vel_configured(m, t, &kern);
+  if (e != cudaSuccess) return e;
+  const int G = 32 / t.lpw, ngroups = (d.wn + G - 1) / G, grid = (ngroups + t.wpb - 1) / t.wpb;
+  kern<<<grid, 32 * t.wpb, t.block_bytes, s>>>(m, d, mask);
   return cudaGetLastError();
+}
+
+cudaError_t resident_worlds_velocity(const ModelDev& m, const DataDev& d, int* worlds) {
+  const TeamShape t = vel_shape(m, d);
+  void (*kern)(ModelDev, DataDev, int);
+  int blocks = 0;
+  cudaError_t e = vel_configured(m, t, &kern);
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, 32 * t.wpb, t.block_bytes);
+  *worlds = blocks * t.wpb * (32 / t.lpw);
+  return e;
 }

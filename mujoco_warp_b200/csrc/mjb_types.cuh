@@ -184,9 +184,12 @@ cudaError_t launch_sensor(const ModelDev& m, const DataDev& d, int stages, cudaS
 cudaError_t launch_contact_force(const ModelDev& m, const DataDev& d, const int* contact_ids, int n, int to_world, float* out, cudaStream_t s);
 cudaError_t launch_rk_stage(const ModelDev& m, const DataDev& d, float* rk, int stage, cudaStream_t s);
 cudaError_t launch_ctrl_noise(const ModelDev& m, const DataDev& d, const float* ctrl_center, int step, float std, float rate, cudaStream_t s);
-size_t smem_position(const ModelDev& m);
+size_t smem_position(const ModelDev& m, const DataDev& d);
 size_t smem_collision(const ModelDev& m, const DataDev& d);
 size_t smem_constraint(const ModelDev& m, const DataDev& d);
-size_t smem_velocity(const ModelDev& m);
+size_t smem_velocity(const ModelDev& m, const DataDev& d);
+// worlds per SM resident at once (occupancy API) in the launch shape k_position / k_velocity take for d's world range
+cudaError_t resident_worlds_position(const ModelDev& m, const DataDev& d, int* worlds);
+cudaError_t resident_worlds_velocity(const ModelDev& m, const DataDev& d, int* worlds);
 size_t smem_solver(const ModelDev& m, const DataDev& d);
 size_t smem_integrate(const ModelDev& m);
