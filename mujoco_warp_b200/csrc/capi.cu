@@ -22,13 +22,6 @@ struct mjbData {
   cudaStream_t aux[8];
   cudaEvent_t ev_fork, ev_join[8];
   int nsplit;
-  cudaStream_t sol_aux[8];        // solver row-capacity classes: second class of each world range runs here
-  cudaEvent_t sol_fork[8], sol_join[8];
-  // fwd_velocity / fwd_actuation / fwd_acceleration need nothing collision or make_constraint write, so inside a world range
-  // k_velocity can run on its own stream next to k_collision -> k_constraint and be joined before the solver (MJB_FORK=1; default serial)
-  cudaStream_t vel_aux[8];
-  cudaEvent_t vel_fork[8], vel_join[8];
-  bool fork_velocity;
   float* rk;  // Runge-Kutta scratch, (nworld, nq + 3 nv + 2 na); allocated by mjb_data_finalize for RK4 models only
 };
 
@@ -118,12 +111,6 @@ void mjb_data_destroy(mjbData* d) {
   if (d->dev.world_conadr) cudaFree(d->dev.world_conadr);
   if (d->dev.world_ncon) cudaFree(d->dev.world_ncon);
   if (d->dev.imp_qacc) cudaFree(d->dev.imp_qacc);
-  if (d->dev.sol_list) cudaFree(d->dev.sol_list);
-  if (d->dev.sol_count) {
-    cudaFree(d->dev.sol_count);
-    for (int i = 0; i < 8; i++) { cudaStreamDestroy(d->sol_aux[i]); cudaEventDestroy(d->sol_fork[i]); cudaEventDestroy(d->sol_join[i]); }
-    for (int i = 0; i < 8; i++) { cudaStreamDestroy(d->vel_aux[i]); cudaEventDestroy(d->vel_fork[i]); cudaEventDestroy(d->vel_join[i]); }
-  }
   if (d->rk) cudaFree(d->rk);
   if (d->nsplit > 1) {
     for (int i = 0; i < d->nsplit; i++) { cudaStreamDestroy(d->aux[i]); cudaEventDestroy(d->ev_join[i]); }
@@ -151,37 +138,12 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
   MJB_DATA_IARRS(X)
 #undef X
   if (d->dev.nv_pad < m->dev.nv) return fail("nv_pad < nv");
-  // nv > 32 solver: Jacobian rows staged in shared memory.  0 (rows are read through L2) by default: the smaller per-world slice lets
-  // more worlds share an SM
-  { const char* e = getenv("MJB_JCAP"); d->dev.jcap = e ? atoi(e) : 0; if (d->dev.jcap < 0) d->dev.jcap = 0; }
   if (check(cudaMalloc(&d->dev.world_conadr, sizeof(int) * (size_t)d->dev.nworld), "cudaMalloc(world_conadr)")) return -1;
   if (check(cudaMalloc(&d->dev.world_ncon, sizeof(int) * (size_t)d->dev.nworld), "cudaMalloc(world_ncon)")) return -1;
   if (check(cudaMemset(d->dev.world_conadr, 0, sizeof(int) * (size_t)d->dev.nworld), "memset")) return -1;
   if (check(cudaMemset(d->dev.world_ncon, 0, sizeof(int) * (size_t)d->dev.nworld), "memset")) return -1;
   // always there (nworld x nv floats), so that switching Option.integrator to the fully implicit one needs no allocation inside a graph capture
   if (check(cudaMalloc(&d->dev.imp_qacc, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nv > 0 ? m->dev.nv : 1)), "cudaMalloc(imp_qacc)")) return -1;
-  if (check(cudaMalloc(&d->dev.sol_list, sizeof(int) * 2 * (size_t)d->dev.nworld), "cudaMalloc(sol_list)")) return -1;
-  if (check(cudaMalloc(&d->dev.sol_count, sizeof(int) * 16), "cudaMalloc(sol_count)")) return -1;
-  if (check(cudaMemset(d->dev.sol_count, 0, sizeof(int) * 16), "memset")) return -1;
-  for (int i = 0; i < 8; i++) {
-    if (check(cudaStreamCreateWithFlags(&d->sol_aux[i], cudaStreamNonBlocking), "cudaStreamCreate")) return -1;
-    if (check(cudaEventCreateWithFlags(&d->sol_fork[i], cudaEventDisableTiming), "cudaEventCreate")) return -1;
-    if (check(cudaEventCreateWithFlags(&d->sol_join[i], cudaEventDisableTiming), "cudaEventCreate")) return -1;
-  }
-  d->dev.sol_stream = d->sol_aux[0]; d->dev.sol_fork = d->sol_fork[0]; d->dev.sol_join = d->sol_join[0];
-  for (int i = 0; i < 8; i++) {
-    if (check(cudaStreamCreateWithFlags(&d->vel_aux[i], cudaStreamNonBlocking), "cudaStreamCreate")) return -1;
-    if (check(cudaEventCreateWithFlags(&d->vel_fork[i], cudaEventDisableTiming), "cudaEventCreate")) return -1;
-    if (check(cudaEventCreateWithFlags(&d->vel_join[i], cudaEventDisableTiming), "cudaEventCreate")) return -1;
-  }
-  {
-    // equality rows read cvel / cdof_dot of the previous step (constraint.py:1085-1117 uses them as they stand when make_constraint
-    // runs), which k_velocity overwrites: models with equalities keep the serial chain
-    const char* e = getenv("MJB_FORK");
-    // off by default: both branches are shared-memory bound, so running them side by side does not raise the number of resident
-    // warps; MJB_FORK=1 enables it (bit-identical results, tested)
-    d->fork_velocity = (e ? atoi(e) != 0 : false) && m->dev.neq == 0 && d->dev.nworld >= 1024;
-  }
   if (m->dev.integrator == INT_RK4 && !d->rk &&
       check(cudaMalloc(&d->rk, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nq + 3 * m->dev.nv + 2 * m->dev.na + 1)), "cudaMalloc(rk)")) return -1;
   d->smem[0] = smem_position(m->dev, d->dev); d->smem[1] = smem_collision(m->dev, d->dev); d->smem[2] = smem_constraint(m->dev, d->dev);
@@ -256,7 +218,7 @@ int mjb_contact_force(const mjbModel* m, mjbData* d, const int* contact_ids, int
 int mjb_sensor_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 1, s), 1); return 0; }
 int mjb_sensor_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 2, s), 1); return 0; }
 int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 4, s), 1); return 0; }
-int mjb_solve(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_solver(m->dev, d->dev, s), solver_launch_count(m->dev, d->dev)); return 0; }
+int mjb_solve(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_solver(m->dev, d->dev, s), 1); return 0; }
 int mjb_euler(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_integrate(m->dev, d->dev, INT_EULER, s), 1); return 0; }
 int mjb_implicit(const mjbModel* m, mjbData* d, void* stream) {
   MJB_ENTER();
@@ -269,25 +231,16 @@ int mjb_implicit(const mjbModel* m, mjbData* d, void* stream) {
 // which stages a pipeline call runs
 enum { RUN_POSITION = 1, RUN_VELOCITY = 2, RUN_SOLVER = 4, RUN_EULER = 8 };
 
-static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int what, cudaStream_t s) {
-  const bool fork = d->fork_velocity && (what & RUN_POSITION) && (what & RUN_VELOCITY);
-  const int h = dd.split_id;
+static int chain(const mjbModel* m, const DataDev& dd, int what, cudaStream_t s) {
   if (what & RUN_POSITION) {
     // forward.py:635-677 with factorize=False: kinematics, com_pos, camlight, crb, collision, make_constraint, transmission
     MJB_LAUNCH(launch_position(m->dev, dd, STG_KINEMATICS | STG_COM_POS | STG_CAMLIGHT | STG_CRB | STG_TRANSMISSION, s), 1);
-    if (fork) {
-      if (check(cudaEventRecord(d->vel_fork[h], s), "cudaEventRecord")) return -1;
-      if (check(cudaStreamWaitEvent(d->vel_aux[h], d->vel_fork[h], 0), "cudaStreamWaitEvent")) return -1;
-      MJB_LAUNCH(launch_velocity(m->dev, dd, STG_VELOCITY | STG_ACTUATION | STG_ACCELERATION, d->vel_aux[h]), 1);
-      if (check(cudaEventRecord(d->vel_join[h], d->vel_aux[h]), "cudaEventRecord")) return -1;
-    }
     MJB_LAUNCH(launch_collision(m->dev, dd, s), 1);
     MJB_LAUNCH(launch_constraint(m->dev, dd, s), 1);
     if (dd.njmax_nnz > 0) MJB_LAUNCH(launch_efc_csr(m->dev, dd, s), 1);  // sparse models: the reference's CSR arrays next to the dense rows
   }
-  if (fork) { if (check(cudaStreamWaitEvent(s, d->vel_join[h], 0), "cudaStreamWaitEvent")) return -1; }
-  else if (what & RUN_VELOCITY) MJB_LAUNCH(launch_velocity(m->dev, dd, STG_VELOCITY | STG_ACTUATION | STG_ACCELERATION, s), 1);
-  if (what & RUN_SOLVER) MJB_LAUNCH(launch_solver(m->dev, dd, s), solver_launch_count(m->dev, dd));
+  if (what & RUN_VELOCITY) MJB_LAUNCH(launch_velocity(m->dev, dd, STG_VELOCITY | STG_ACTUATION | STG_ACCELERATION, s), 1);
+  if (what & RUN_SOLVER) MJB_LAUNCH(launch_solver(m->dev, dd, s), 1);
   // sensors of all three stages in one launch after the solver (forward.py:1350-1365 interleaves them; their inputs are final by now)
   if ((what & RUN_SOLVER) && m->dev.nsensor > 0) MJB_LAUNCH(launch_sensor(m->dev, dd, 7, s), 1);
   if (what & RUN_EULER) {
@@ -299,7 +252,7 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
 
 static int pipeline(const mjbModel* m, mjbData* d, int what, cudaStream_t s) {
   if (what & RUN_POSITION) MJB_LAUNCH(reset_contact_counters(d->dev, s), 0);
-  if (d->nsplit < 2) return chain(m, d, d->dev, what, s);
+  if (d->nsplit < 2) return chain(m, d->dev, what, s);
   // fork: both halves wait for everything queued on the caller's stream, run their own kernel chain, and are joined back
   if (check(cudaEventRecord(d->ev_fork, s), "cudaEventRecord")) return -1;
   const int part = (d->dev.nworld + d->nsplit - 1) / d->nsplit;
@@ -307,11 +260,9 @@ static int pipeline(const mjbModel* m, mjbData* d, int what, cudaStream_t s) {
     DataDev dd = d->dev;
     dd.w0 = h * part;
     dd.wn = min(part, d->dev.nworld - dd.w0);
-    dd.split_id = h;
-    dd.sol_stream = d->sol_aux[h]; dd.sol_fork = d->sol_fork[h]; dd.sol_join = d->sol_join[h];
     if (dd.wn <= 0) break;
     if (check(cudaStreamWaitEvent(d->aux[h], d->ev_fork, 0), "cudaStreamWaitEvent")) return -1;
-    if (chain(m, d, dd, what, d->aux[h])) return -1;
+    if (chain(m, dd, what, d->aux[h])) return -1;
     if (check(cudaEventRecord(d->ev_join[h], d->aux[h]), "cudaEventRecord")) return -1;
     if (check(cudaStreamWaitEvent(s, d->ev_join[h], 0), "cudaStreamWaitEvent")) return -1;
   }

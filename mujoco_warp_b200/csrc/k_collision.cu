@@ -15,7 +15,6 @@
 // pool layout (types.py:1975-2018) so [0, nacon) is densely packed.
 #include "mjb_ccd.cuh"
 #include "mjb_colliders.cuh"
-#include <cstdlib>
 
 #include "mjb_math.cuh"
 #include "mjb_team.cuh"
@@ -491,12 +490,8 @@ k_collision(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev
 
 }  // namespace
 
-// warps (= worlds) per block: one-warp blocks cap an SM at 32 resident worlds (CTA limit); MJB_WPB_COL overrides
-static int collision_wpb() {
-  static int v = 0;
-  if (!v) { const char* e = getenv("MJB_WPB_COL"); v = e ? atoi(e) : 2; if (v < 1 || v > 2) v = 2; }
-  return v;
-}
+// warps (= worlds) per block: one-warp blocks cap an SM at 32 resident worlds (CTA limit)
+constexpr int collision_wpb() { return 2; }
 
 #ifdef MJB_COLLISION_MESH_TU
 #define LAUNCH_NAME launch_collision_mesh

@@ -11,7 +11,6 @@
 // atomics-dependent; its own tests sort before comparing, constraint_test.py:40-59).  Lanes map to dofs: a J row is a
 // single coalesced store, J*qvel is a warp-shuffle reduction; the per-row impedance / reference math of the contact rows runs
 // afterwards with lanes = rows of the 32-contact batch (phase C), so its eight per-row stores are coalesced over consecutive rows.
-#include <cstdlib>
 
 #include "mjb_math.cuh"
 #include "mjb_types.cuh"
@@ -543,12 +542,8 @@ k_constraint(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDe
 
 }  // namespace
 
-// warps (= worlds) per block: one-warp blocks cap an SM at 32 resident worlds (CTA limit); MJB_WPB_CON overrides
-static int constraint_wpb() {
-  static int v = 0;
-  if (!v) { const char* e = getenv("MJB_WPB_CON"); v = e ? atoi(e) : 2; if (v < 1 || v > 2) v = 2; }
-  return v;
-}
+// warps (= worlds) per block: one-warp blocks cap an SM at 32 resident worlds (CTA limit)
+constexpr int constraint_wpb() { return 2; }
 
 size_t smem_constraint(const ModelDev& m, const DataDev& d) { return (size_t)con_layout(m, d).total * sizeof(float) * constraint_wpb(); }
 

@@ -7,7 +7,6 @@
 // parents gather their children in fixed order (deterministic; no float atomics), and every Data field is written
 // once with coalesced row stores.  `mask` selects sub-stages so each public stage function stays individually callable;
 // inputs a skipped sub-stage would have produced are re-loaded from Data.
-#include <cstdlib>
 
 #include "mjb_math.cuh"
 #include "mjb_team.cuh"
@@ -400,11 +399,11 @@ k_position(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
 }  // namespace
 
 static void (*pos_kernel(const ModelDev& m, int lpw))(ModelDev, DataDev, int) {
-  return m.batched ? k_position<32, true> : lpw == 4 ? k_position<4, false> : lpw == 8 ? k_position<8, false> : lpw == 16 ? k_position<16, false> : k_position<32, false>;
+  return m.batched ? k_position<32, true> : lpw == 8 ? k_position<8, false> : lpw == 16 ? k_position<16, false> : k_position<32, false>;
 }
 
 static TeamShape pos_shape(const ModelDev& m, const DataDev& d) {
-  TeamShape t = team_shape((size_t)pos_layout(m).total, d.wn, "MJB_LPW_POS", "MJB_WPB_POS", [&](int lpw) { return kernel_regs(pos_kernel(m, lpw)); });
+  TeamShape t = team_shape((size_t)pos_layout(m).total, d.wn, [&](int lpw) { return kernel_regs(pos_kernel(m, lpw)); });
   if (m.batched && t.lpw != 32) { t = team_shape_fixed((size_t)pos_layout(m).total, 32, 2); }
   return t;
 }
@@ -412,8 +411,8 @@ size_t smem_position(const ModelDev& m, const DataDev& d) { return pos_shape(m, 
 
 // the kernel instance for the launch shape, configured on its first use
 static cudaError_t pos_configured(const ModelDev& m, const TeamShape& t, void (**kern)(ModelDev, DataDev, int)) {
-  static TeamConfig configured[5];
-  const int lpw = t.lpw, ki = m.batched ? 4 : lpw == 4 ? 0 : lpw == 8 ? 1 : lpw == 16 ? 2 : 3;
+  static TeamConfig configured[4];
+  const int lpw = t.lpw, ki = m.batched ? 3 : lpw == 8 ? 0 : lpw == 16 ? 1 : 2;
   *kern = pos_kernel(m, lpw);
   return team_configure(*kern, t.block_bytes, &configured[ki]);
 }

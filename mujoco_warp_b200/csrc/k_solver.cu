@@ -1,5 +1,5 @@
-// k_solver.cu -- Newton constraint solver as ONE persistent launch (one warp per world -- a team of 2 or 4 warps above
-// nv = 32 -- with all state in shared memory).
+// k_solver.cu -- Newton constraint solver as ONE persistent launch (one warp per world, with all state in shared memory
+// except, above nv = 32, the Jacobian rows, which are read through L2).
 //
 // Replaces (reference, /root/reference/mujoco_warp/_src/solver.py): :3671 solve / :3689 _solve, :3622 init_context,
 // :1566 _solve_init_dof, :1609 _solve_init_jaref, support.py:153 mul_m, :1698 _update_constraint_efc,
@@ -15,8 +15,6 @@
 // shifted (cost(alpha) - cost(0)) piecewise-quadratic 1-D cost.  Pyramidal / frictionless / limit / dof-friction rows
 // in the default instantiation; k_solver<true> adds elliptic cones (solver.py:286-477 zones, :957-1015 per-contact
 // quads, :2443-2565 cone Hessian) with the Hessian rebuilt from M every iteration like the reference's elliptic path.
-#include <cstdlib>
-
 #include "mjb_chol.cuh"
 #include "mjb_linesearch.cuh"
 #include "mjb_team.cuh"
@@ -28,28 +26,24 @@ namespace {
 // Shared-memory slice of one world.  J rows keep the global stride nv_pad (a multiple of 4 floats), so a row is 16-byte
 // aligned: staging is a straight float4 copy and row-times-vector products use LDS.128 (a quarter-warp of 112-byte-strided
 // rows is bank-conflict free).  Per-dof vectors are padded to nv_pad with zeros so the float4 loops need no tail handling.
-struct SolLayout { int J, vec, H, Lf, M, rowf, rowi, ldJ, ldH, nvp, nrowf, jcap, cgv, red, env, bar, total; };
-// rows of shared memory a world gets: d.rowcap for a row-capacity class launch (see launch_solver), else njmax
-__host__ __device__ inline int sol_rowcap(const DataDev& d) { return d.rowcap > 0 ? d.rowcap : d.njmax; }
+struct SolLayout { int J, vec, H, Lf, M, rowf, rowi, ldJ, ldH, nvp, nrowf, cgv, env, bar, total; };
 __host__ __device__ inline SolLayout sol_layout(const ModelDev& m, const DataDev& d, bool big) {
   SolLayout L;
-  const int cap = sol_rowcap(d);
+  const int cap = d.njmax;
   int o = 0;
   auto take = [&](int n) { int r = o; o += (n + 3) & ~3; return r; };
   L.nvp = d.nv_pad; L.ldJ = d.nv_pad; L.ldH = m.nv | 1;
-  // nv > 32 ("big" models, e.g. unitree G1, three_humanoids): only the first d.jcap Jacobian rows are staged in shared memory,
-  // the rest is read from global memory (L2 hits).  d.jcap defaults to 0: occupancy beats the shorter access (see capi.cu).
-  L.jcap = big ? (cap < d.jcap ? cap : d.jcap) : cap;
-  L.J = take(L.jcap * L.ldJ);
+  // nv > 32 ("big" models, e.g. unitree G1, three_humanoids): no Jacobian rows are staged, they are read from global memory (L2
+  // hits) -- the smaller slice lets more worlds share an SM, which beats the shorter access
+  L.J = take(big ? 0 : cap * L.ldJ);
   L.vec = take(7 * L.nvp);  // qacc, Ma, grad, search, mv (= x scratch of the nv > 32 path), qfs, qfc
   L.cgv = take(m.solver == SOL_CG ? 3 * L.nvp : 0);  // CG only: Mgrad, prev_grad, prev_Mgrad
-  // nv <= 32: H and its factor are stored as packed lower triangles (register Cholesky path); larger nv keeps nv x ldH
   // H and its factor are packed lower triangles (register Cholesky for nv <= 32, shared-memory Cholesky above)
   const int hsz = m.nv * (m.nv + 1) / 2;
   L.H = take(hsz);
-  // nv <= 32: the factor lives in the padded column layout of chol_solve_rows_bcast, and M is kept as a dense packed lower
+  // nv <= 32: the factor lives in the paired-column layout of chol_solve_rows_pair, and M is kept as a dense packed lower
   // triangle (H starts as a copy of it, M * v needs no index tables); nv > 32: packed factor, CSR M with gather tables
-  L.Lf = take(big ? hsz : cholpair_size(m.nv <= 8 ? 8 : m.nv <= 16 ? 16 : m.nv <= 24 ? 24 : m.nv <= 28 ? 28 : 32));  // padded size of the register path (>= colsub_off of the same size)
+  L.Lf = take(big ? hsz : cholpair_size(m.nv <= 8 ? 8 : m.nv <= 16 ? 16 : m.nv <= 24 ? 24 : m.nv <= 28 ? 28 : 32));  // padded size of the register path
   L.M = take(big ? m.nC : hsz);
   // Jaref, jv (= hw: the H-update weights live only between update_constraint and update_search), D, force [, floss]
   // elliptic cones add: per-row friction scale, 3 quad words per row (solver.py:1008-1015 layout), row->contact info
@@ -57,7 +51,6 @@ __host__ __device__ inline SolLayout sol_layout(const ModelDev& m, const DataDev
   L.nrowf = ((m.nfricdof + m.ntenfric) > 0 ? 5 : 4);
   L.rowf = take((L.nrowf + (ell ? 4 : 0)) * cap);
   L.rowi = take((ell ? 3 : 2) * cap);
-  L.red = take(big ? 9 * 8 : 0);  // cross-warp reduction scratch of the multi-warp (nv > 32) instantiations
   // nv > 32: nonzero column range of every Jacobian row (lo | hi << 16) and the Hessian's row envelope (first column per row)
   L.env = take(big ? cap + L.nvp : 0);
   L.bar = take(4);  // mbarrier of the bulk-async staging (8 bytes, 16-byte slot)
@@ -65,35 +58,10 @@ __host__ __device__ inline SolLayout sol_layout(const ModelDev& m, const DataDev
   return L;
 }
 
-// ---- team = the NW warps (one block) that own a world.  NW = 1: plain warp primitives.  NW > 1 (models with nv > 32, where a
-// world's slice of shared memory caps the SM at a few resident worlds): block barriers, and reductions that finish in shared
-// memory in a fixed order so every thread sees the same bits.
-template <int NW> __device__ __forceinline__ void tsync() { if (NW == 1) __syncwarp(); else __syncthreads(); }
-template <int NW, int N>
-__device__ __forceinline__ void tsum_n(float (&v)[N], float* red) {
-#pragma unroll
-  for (int k = 0; k < N; k++) v[k] = warp_sum(v[k]);
-  if (NW == 1) return;
-  const int warp = threadIdx.x >> 5;
-  __syncthreads();  // the previous reduction's readers are done with `red`
-  if ((threadIdx.x & 31) == 0) {
-#pragma unroll
-    for (int k = 0; k < N; k++) red[warp * N + k] = v[k];
-  }
-  __syncthreads();
-#pragma unroll
-  for (int k = 0; k < N; k++) {
-    float t = red[k];
-#pragma unroll
-    for (int w = 1; w < NW; w++) t += red[w * N + k];
-    v[k] = t;
-  }
-}
-template <int NW> __device__ __forceinline__ float tsum(float v, float* red) { float a[1] = {v}; tsum_n<NW, 1>(a, red); return a[0]; }
-template <int NW> __device__ __forceinline__ P3 tsum3(P3 p, float* red) { float a[3] = {p.c, p.g, p.h}; tsum_n<NW, 3>(a, red); return mkp(a[0], a[1], a[2]); }
-template <int NW> __device__ __forceinline__ void tcopy(float* dst, const float* src, int n, int tid) {
+__device__ __forceinline__ P3 warp_sum3(P3 p) { return mkp(warp_sum(p.c), warp_sum(p.g), warp_sum(p.h)); }
+__device__ __forceinline__ void tcopy(float* dst, const float* src, int n, int lane) {
 #pragma unroll 1  // n is a per-dof count: one or two trips; the unrolled-by-16 form the compiler picks costs ~45 instructions per call (solver 206 -> 202 us)
-  for (int i = tid; i < n; i += 32 * NW) dst[i] = src[i];
+  for (int i = lane; i < n; i += 32) dst[i] = src[i];
 }
 
 // dot of a 16B-aligned J row with a zero-padded, 16B-aligned per-dof vector
@@ -117,9 +85,8 @@ struct Ctx {
   // elliptic only: rinfo[r] = -1 (not an elliptic row) | -2 (contact cut by njmax) | (dim << 4) | j;  rfri[r] = mu (j = 0)
   // or friction[j-1];  quad = 3 words per row;  the CONE contacts' primary rows are listed from the END of hidx
   int* rinfo; float *rfri, *quad; int njmax, ncone;
-  const float* Jg; int jcap;  // big models: rows >= jcap live in global memory (same leading dimension)
+  const float* Jg;            // the world's Jacobian in global memory (same leading dimension): big models read their rows here
   float* cgv;                 // CG only: Mgrad, prev_grad, prev_Mgrad (nvp each)
-  float* red;                 // NW > 1: cross-warp reduction scratch (9 floats per warp)
   int *rng, *fz;              // nv > 32: Jacobian row ranges, Hessian row envelope
   bool env;                   // ranges / envelope in use (several kinematic trees: the Hessian is close to block diagonal)
   float chol_inv;             // nv <= 32: lane j keeps 1 / L_jj of the factor in Lf
@@ -128,7 +95,7 @@ struct Ctx {
 };
 template <bool BIG>
 __device__ __forceinline__ const float* jrow(const Ctx& c, int r) {
-  if (BIG && r >= c.jcap) return c.Jg + (size_t)r * c.ldJ;
+  if (BIG) return c.Jg + (size_t)r * c.ldJ;
   return c.J + r * c.ldJ;
 }
 __device__ __forceinline__ EllQ ell_load(const Ctx& c, int r) {
@@ -141,7 +108,7 @@ __device__ __forceinline__ EllQ ell_load(const Ctx& c, int r) {
 // diagonal and column i below it -- no index tables, no global loads (the CSR gather's table lookups were the top long-scoreboard line
 // of the solver).  A fully unrolled variant with predicated loads (4 instead of 9 instructions per entry) measured SLOWER: 245 vs 206 us.
 // nv > 32: the symmetric gather tables (io.py:1029-1050).
-template <int NW, bool BIG>
+template <bool BIG>
 __device__ __forceinline__ void mul_m(const Ctx& c, const float* vec, float* res) {
   const ModelDev& m = *c.m;
   if (!BIG) {
@@ -158,26 +125,26 @@ __device__ __forceinline__ void mul_m(const Ctx& c, const float* vec, float* res
       }
       res[i] = acc;
     }
-    return;
-  }
+  } else {
 #pragma unroll 1
-  for (int i = c.lane; i < c.nv; i += 32 * NW) {
-    float acc = 0.f;
+    for (int i = c.lane; i < c.nv; i += 32) {
+      float acc = 0.f;
 #pragma unroll 4
-    for (int k = m.mulm_rowadr[i]; k < m.mulm_rowadr[i + 1]; k++) acc += c.M[m.mulm_madr[k]] * vec[m.mulm_col[k]];
-    res[i] = acc;
+      for (int k = m.mulm_rowadr[i]; k < m.mulm_rowadr[i + 1]; k++) acc += c.M[m.mulm_madr[k]] * vec[m.mulm_col[k]];
+      res[i] = acc;
+    }
   }
 }
 
 // force/state per row, qfrc_constraint = J^T force, and the list of rows whose QUADRATIC flag changed
 // (init=true: list every QUADRATIC row with weight +D).  Returns the list length.
-template <bool ELL, bool BIG, int NW>
+template <bool ELL, bool BIG>
 __device__ __forceinline__ int update_constraint(Ctx& c, bool init) {
   int nlist = 0, ncone = 0;
   if (ELL) init = true;  // elliptic: H is rebuilt from M, so every QUADRATIC row is listed
-  // the row pass (a handful of flops per row, ordered compaction by ballot) stays on the first warp of the team
+  // the row pass: a handful of flops per row, ordered compaction by ballot
 #pragma unroll 1
-  for (int r0 = 0; r0 < ((NW == 1 || c.lane < 32) ? c.nefc : 0); r0 += 32) {
+  for (int r0 = 0; r0 < c.nefc; r0 += 32) {
     const int r = r0 + c.lane;
     bool flip = false, cone0 = false;
     float wgt = 0.f;
@@ -223,32 +190,26 @@ __device__ __forceinline__ int update_constraint(Ctx& c, bool init) {
       ncone += __popc(cb);
     }
   }
-  if (NW > 1) {  // hand the two counts to the other warps
-    if (c.lane == 0) { c.red[0] = __int_as_float(nlist); c.red[1] = __int_as_float(ncone); }
-    __syncthreads();
-    nlist = __float_as_int(c.red[0]); ncone = __float_as_int(c.red[1]);
-  }
   c.ncone = ncone;
-  tsync<NW>();
+  __syncwarp();
 #pragma unroll 1
-  for (int dd = c.lane; dd < c.nv; dd += 32 * NW) {
+  for (int dd = c.lane; dd < c.nv; dd += 32) {
     float s = 0.f;
 #pragma unroll 8
     for (int r = 0; r < c.nefc; r++) s += jrow<BIG>(c, r)[dd] * c.force[r];
     c.qfc[dd] = s;
   }
-  tsync<NW>();
+  __syncwarp();
   return nlist;
 }
 
 // grad = Ma - qfrc_smooth - qfrc_constraint and its squared norm
-template <int NW>
 __device__ __forceinline__ void update_grad(Ctx& c) {
   float gd = 0.f;
 #pragma unroll 1
-  for (int dd = c.lane; dd < c.nv; dd += 32 * NW) { const float g = c.Ma[dd] - c.qfs[dd] - c.qfc[dd]; c.grad[dd] = g; gd += g * g; }
-  c.grad_dot = tsum<NW>(gd, c.red);
-  tsync<NW>();
+  for (int dd = c.lane; dd < c.nv; dd += 32) { const float g = c.Ma[dd] - c.qfs[dd] - c.qfc[dd]; c.grad[dd] = g; gd += g * g; }
+  c.grad_dot = warp_sum(gd);
+  __syncwarp();
 }
 
 // Newton direction for nv <= 32: lane i keeps row i of H in registers, adds w * J_r[i] * J_r[:] for every listed row r
@@ -323,20 +284,12 @@ __device__ __forceinline__ float newton_direction_reg(Ctx& c, int nlist, float g
       }
     }
   }
-#ifdef MJB_CHOL_UNROLLED  // off by default: the straight-line sweep misses the instruction cache (see mjb_chol.cuh)
-  return chol_solve_rows_unrolled<N>(a, nv, g, c.Lf, lane);
-#else
   c.factored = true;
-#ifdef MJB_CHOL_SINGLE  // one column per sweep (humanoid solver 216 us)
-  return chol_solve_rows_bcast<N>(a, nv, g, c.Lf, lane, c.chol_inv);
-#else
   return chol_solve_rows_pair<N>(a, nv, g, c.Lf, lane, c.chol_inv, c.chol_off);
-#endif
-#endif
 }
 
 // H += sum_list w J J^T (lower triangle), Cholesky, search = -H^-1 grad, Newton decrement
-template <bool ELL, bool BIG, int NW, int NREG = 0>
+template <bool ELL, bool BIG, int NREG = 0>
 __device__ __forceinline__ void update_search(Ctx& c, int nlist) {
   const int nv = c.nv;
   float sd = 0.f, nd = 0.f;
@@ -345,11 +298,7 @@ __device__ __forceinline__ void update_search(Ctx& c, int nlist) {
     float xx;
     // no row changed state since the last factorisation: H is what was factored, only the right-hand side is new (the reference's
     // stable-state shortcut, solver.py:2145-2159, which reuses the whole direction instead)
-#ifdef MJB_CHOL_SINGLE
-    if (!ELL && nlist == 0 && c.factored) xx = chol_subst_bcast(nv, g, c.Lf, c.lane, c.chol_inv);
-#else
     if (!ELL && nlist == 0 && c.factored) xx = chol_subst_pair(nv, g, c.Lf, c.lane, c.chol_inv, c.chol_off);
-#endif
     else if (NREG == 28) xx = newton_direction_reg<28, ELL>(c, nlist, g);  // register-row size fixed by the launcher: one variant in the kernel
     else if (NREG == 32) xx = newton_direction_reg<32, ELL>(c, nlist, g);
     else if (nv <= 8) xx = newton_direction_reg<8, ELL>(c, nlist, g);
@@ -360,45 +309,30 @@ __device__ __forceinline__ void update_search(Ctx& c, int nlist) {
     sd = xx * xx; nd = g * xx;
     if (c.lane < nv) c.search[c.lane] = -xx;
   } else {
-    // nv > 32: packed lower triangle in shared memory, worked on by the whole team
-    constexpr int NT = 32 * NW;
+    // nv > 32: packed lower triangle in shared memory; lane owns rows lane, lane + 32, ...
     const int ntri = nv * (nv + 1) / 2;
     float* Hd = ELL ? c.Lf : c.H;  // elliptic: rebuild into Lf from M (c.H) every iteration
     if (ELL) {
 #pragma unroll 1
-      for (int e = c.lane; e < ntri; e += NT) c.Lf[e] = c.H[e];
-      tsync<NW>();
+      for (int e = c.lane; e < ntri; e += 32) c.Lf[e] = c.H[e];
+      __syncwarp();
     }
-    if (NW == 1) {  // one warp: lane owns rows lane, lane + 32, ...
 #pragma unroll 1
-      for (int t = 0; t < nlist; t++) {
-        const float* Jr = jrow<true>(c, c.hidx[t]);
-        const float wt = c.hw[t];
-        const int lo = c.env ? (c.rng[c.hidx[t]] & 0xFFFF) : 0, hi = c.env ? (c.rng[c.hidx[t]] >> 16) : nv;  // the row is zero outside [lo, hi)
+    for (int t = 0; t < nlist; t++) {
+      const float* Jr = jrow<true>(c, c.hidx[t]);
+      const float wt = c.hw[t];
+      const int lo = c.env ? (c.rng[c.hidx[t]] & 0xFFFF) : 0, hi = c.env ? (c.rng[c.hidx[t]] >> 16) : nv;  // the row is zero outside [lo, hi)
 #pragma unroll 1
-        for (int i = lo + ((c.lane - lo) & 31); i < hi; i += 32) {  // row i always belongs to lane i % 32, whatever the row range
-          const float sc = wt * Jr[i];
-          float* Hi = Hd + (i * (i + 1)) / 2;
-          if (sc != 0.f)
+      for (int i = lo + ((c.lane - lo) & 31); i < hi; i += 32) {  // row i always belongs to lane i % 32, whatever the row range
+        const float sc = wt * Jr[i];
+        float* Hi = Hd + (i * (i + 1)) / 2;
+        if (sc != 0.f)
 #pragma unroll 4
-            for (int k = lo; k <= i; k++) Hi[k] += sc * Jr[k];
-        }
-      }
-    } else if (nlist > 0) {  // team: every thread owns entries (i, k) of the triangle and sums the listed rows' contributions
-#pragma unroll 1
-      for (int e = c.lane; e < ntri; e += NT) {
-        int i = (int)((sqrtf(8.0f * (float)e + 1.0f) - 1.0f) * 0.5f);
-        while ((i + 1) * (i + 2) / 2 <= e) i++;
-        while (i * (i + 1) / 2 > e) i--;
-        const int k = e - i * (i + 1) / 2;
-        float acc = 0.f;
-#pragma unroll 4
-        for (int t = 0; t < nlist; t++) { const float* Jr = jrow<true>(c, c.hidx[t]); acc += c.hw[t] * Jr[i] * Jr[k]; }
-        Hd[e] += acc;
+          for (int k = lo; k <= i; k++) Hi[k] += sc * Jr[k];
       }
     }
     if (ELL) {
-      tsync<NW>();
+      __syncwarp();
 #pragma unroll 1
       for (int t = 0; t < c.ncone; t++) {
         const int e0 = c.hidx[c.njmax - 1 - t];
@@ -406,7 +340,7 @@ __device__ __forceinline__ void update_search(Ctx& c, int nlist) {
         if (k.dm == 0.f) continue;
         const float* J0 = jrow<true>(c, e0);
 #pragma unroll 1
-        for (int i = c.lane; i < nv; i += NT) {
+        for (int i = c.lane; i < nv; i += 32) {
           float pi = 0.f;
           for (int q = 1; q < k.dim; q++) pi += c.Jaref[e0 + q] * c.rfri[e0 + q] * c.rfri[e0 + q] * jrow<true>(c, e0 + q)[i];
           float* Hi = Hd + (i * (i + 1)) / 2;
@@ -418,63 +352,57 @@ __device__ __forceinline__ void update_search(Ctx& c, int nlist) {
         }
       }
     }
-    tsync<NW>();
+    __syncwarp();
     if (!ELL) {
 #pragma unroll 1
-      for (int e = c.lane; e < ntri; e += NT) c.Lf[e] = c.H[e];
+      for (int e = c.lane; e < ntri; e += 32) c.Lf[e] = c.H[e];
     }
 #pragma unroll 1
-    for (int dd = c.lane; dd < nv; dd += NT) c.x[dd] = c.grad[dd];
-    tsync<NW>();
-    if (NW == 1) {
-      if (c.env) {
-        warp_cholesky_packed_env(c.Lf, nv, c.fz, c.lane);
-        warp_chol_solve_packed_env(c.Lf, nv, c.fz, c.x, c.lane);
-      } else {
-        warp_cholesky_packed(c.Lf, nv, c.lane);
-        warp_chol_solve_packed(c.Lf, nv, c.x, c.lane);
-      }
+    for (int dd = c.lane; dd < nv; dd += 32) c.x[dd] = c.grad[dd];
+    __syncwarp();
+    if (c.env) {
+      warp_cholesky_packed_env(c.Lf, nv, c.fz, c.lane);
+      warp_chol_solve_packed_env(c.Lf, nv, c.fz, c.x, c.lane);
     } else {
-      team_cholesky_packed<NW>(c.Lf, nv, c.lane);
-      team_chol_solve_packed<NW>(c.Lf, nv, c.x, c.lane);
+      warp_cholesky_packed(c.Lf, nv, c.lane);
+      warp_chol_solve_packed(c.Lf, nv, c.x, c.lane);
     }
 #pragma unroll 1
-    for (int dd = c.lane; dd < nv; dd += NT) { const float xx = c.x[dd]; sd += xx * xx; nd += c.grad[dd] * xx; c.search[dd] = -xx; }
+    for (int dd = c.lane; dd < nv; dd += 32) { const float xx = c.x[dd]; sd += xx * xx; nd += c.grad[dd] * xx; c.search[dd] = -xx; }
   }
-  { float a[2] = {sd, nd}; tsum_n<NW, 2>(a, c.red); c.search_dot = a[0]; c.newton_decrement = a[1]; }
-  tsync<NW>();
+  c.search_dot = warp_sum(sd); c.newton_decrement = warp_sum(nd);
+  __syncwarp();
 }
 
-template <bool ELL, int NW>
+template <bool ELL>
 __device__ __forceinline__ P3 eval_total(const Ctx& c, float alpha, float q0, float q1, float q2) {
   P3 s = mkp(0.f, 0.f, 0.f);
 #pragma unroll 1
-  for (int r = c.lane; r < c.nefc; r += 32 * NW) {
+  for (int r = c.lane; r < c.nefc; r += 32) {
     if (ELL && c.rinfo[r] != -1) {
       if (c.rinfo[r] >= 0 && (c.rinfo[r] & 15) == 0) { const EllQ q = ell_load(c, r); const float mu = c.rfri[r]; s = s + ell_shifted(mu, q, ell_reference(mu, q), alpha); }
     } else s = s + eval_row(r, alpha, c.ne, c.nf, c.D[r], c.floss[r], c.Jaref[r], c.jv[r]);
   }
-  return eval_gauss(q0, q1, q2, alpha) + tsum3<NW>(s, c.red);
+  return eval_gauss(q0, q1, q2, alpha) + warp_sum3(s);
 }
 
 // solver.py:836-1347; returns true when the line search converged
-template <bool ELL, bool BIG, int NW>
+template <bool ELL, bool BIG>
 __device__ __forceinline__ bool linesearch(Ctx& c) {
   const ModelDev& m = *c.m;
   const int nv = c.nv;
-  constexpr int NT = 32 * NW;
-  mul_m<NW, BIG>(c, c.search, c.mv);
+  mul_m<BIG>(c, c.search, c.mv);
 #pragma unroll 1
-  for (int r = c.lane; r < c.nefc; r += NT) {
+  for (int r = c.lane; r < c.nefc; r += 32) {
     c.jv[r] = row_dot(jrow<BIG>(c, r), c.search, c.nvp);
   }
-  tsync<NW>();
+  __syncwarp();
   const float snorm = sqrtf(c.search_dot), scale = m.meaninertia * (float)nv;
   const float gtol = fmaxf(m.tolerance * m.ls_tolerance * snorm * scale, 1e-6f);
   P3 p0s = mkp(0.f, 0.f, 0.f);
   if (ELL) {  // per-contact quads at the primary rows (solver.py:957-1015)
 #pragma unroll 1
-    for (int r = c.lane; r < c.nefc; r += NT) {
+    for (int r = c.lane; r < c.nefc; r += 32) {
       const int info = c.rinfo[r];
       if (info < 0 || (info & 15) != 0) continue;
       const int dim = info >> 4;
@@ -490,24 +418,23 @@ __device__ __forceinline__ bool linesearch(Ctx& c) {
       const float mu2 = mu * mu;
       q[0] = q0; q[1] = q1; q[2] = q2; q[3] = ja * mu; q[4] = jv * mu; q[5] = uu; q[6] = uv; q[7] = vv; q[8] = D / (mu2 * (1.0f + mu2));
     }
-    tsync<NW>();
+    __syncwarp();
   }
 #pragma unroll 1
-  for (int r = c.lane; r < c.nefc; r += NT) {
+  for (int r = c.lane; r < c.nefc; r += 32) {
     if (ELL && c.rinfo[r] != -1) {
       if (c.rinfo[r] >= 0 && (c.rinfo[r] & 15) == 0) p0s = p0s + ell_zero(c.rfri[r], ell_load(c, r));
     } else p0s = p0s + eval_row_zero(r, c.ne, c.nf, c.D[r], c.floss[r], c.Jaref[r], c.jv[r]);
   }
   float g1 = 0.f, g2 = 0.f;
 #pragma unroll 1
-  for (int dd = c.lane; dd < nv; dd += NT) { const float s = c.search[dd]; g1 += s * (c.Ma[dd] - c.qfs[dd]); g2 += 0.5f * s * c.mv[dd]; }
-  float q1, q2;
-  { float a[5] = {p0s.c, p0s.g, p0s.h, g1, g2}; tsum_n<NW, 5>(a, c.red); p0s = mkp(a[0], a[1], a[2]); q1 = a[3]; q2 = a[4]; }
-  const float q0 = 0.f;
+  for (int dd = c.lane; dd < nv; dd += 32) { const float s = c.search[dd]; g1 += s * (c.Ma[dd] - c.qfs[dd]); g2 += 0.5f * s * c.mv[dd]; }
+  p0s = warp_sum3(p0s);
+  const float q0 = 0.f, q1 = warp_sum(g1), q2 = warp_sum(g2);
   const P3 p0 = mkp(q0 + p0s.c, q1 + p0s.g, 2.0f * q2 + p0s.h);
   const P3 p0_delta = mkp(0.f, p0.g, p0.h);
   const float lo_alpha_in = -safe_div(p0.g, p0.h);
-  const P3 lo_in = eval_total<ELL, NW>(c, lo_alpha_in, q0, q1, q2);
+  const P3 lo_in = eval_total<ELL>(c, lo_alpha_in, q0, q1, q2);
   const bool initial_converged = fabsf(lo_in.g) < gtol && lo_in.c < 0.f;
   bool ls_converged = initial_converged;
   float alpha = 0.f, improvement = 0.f;
@@ -520,7 +447,7 @@ __device__ __forceinline__ bool linesearch(Ctx& c) {
       const float lo_next_alpha = lo_alpha - safe_div(lo.g, lo.h), hi_next_alpha = hi_alpha - safe_div(hi.g, hi.h), mid_alpha = 0.5f * (lo_alpha + hi_alpha);
       P3 sl = mkp(0.f, 0.f, 0.f), sh = sl, sm = sl;
 #pragma unroll 1
-      for (int r = c.lane; r < c.nefc; r += NT) {
+      for (int r = c.lane; r < c.nefc; r += 32) {
         if (ELL && c.rinfo[r] != -1) {
           if (c.rinfo[r] >= 0 && (c.rinfo[r] & 15) == 0) {
             const EllQ q = ell_load(c, r); const float mu = c.rfri[r]; const EllRef e = ell_reference(mu, q);
@@ -533,14 +460,9 @@ __device__ __forceinline__ bool linesearch(Ctx& c) {
         sh = sh + eval_row(r, hi_next_alpha, c.ne, c.nf, D, f, ja, jv);
         sm = sm + eval_row(r, mid_alpha, c.ne, c.nf, D, f, ja, jv);
       }
-      {
-        float a[9] = {sl.c, sl.g, sl.h, sh.c, sh.g, sh.h, sm.c, sm.g, sm.h};
-        tsum_n<NW, 9>(a, c.red);
-        sl = mkp(a[0], a[1], a[2]); sh = mkp(a[3], a[4], a[5]); sm = mkp(a[6], a[7], a[8]);
-      }
-      const P3 lo_next = eval_gauss(q0, q1, q2, lo_next_alpha) + sl;
-      const P3 hi_next = eval_gauss(q0, q1, q2, hi_next_alpha) + sh;
-      const P3 mid = eval_gauss(q0, q1, q2, mid_alpha) + sm;
+      const P3 lo_next = eval_gauss(q0, q1, q2, lo_next_alpha) + warp_sum3(sl);
+      const P3 hi_next = eval_gauss(q0, q1, q2, hi_next_alpha) + warp_sum3(sh);
+      const P3 mid = eval_gauss(q0, q1, q2, mid_alpha) + warp_sum3(sm);
       const bool s1 = in_bracket(lo, lo_next); if (s1) { lo = lo_next; lo_alpha = lo_next_alpha; }
       const bool s2 = in_bracket(lo, mid); if (s2) { lo = mid; lo_alpha = mid_alpha; }
       const bool s3 = in_bracket(lo, hi_next); if (s3) { lo = hi_next; lo_alpha = hi_next_alpha; }
@@ -557,11 +479,11 @@ __device__ __forceinline__ bool linesearch(Ctx& c) {
     alpha = lo_alpha_in; improvement = -lo_in.c;
   }
 #pragma unroll 1
-  for (int dd = c.lane; dd < nv; dd += NT) { c.qacc[dd] += alpha * c.search[dd]; c.Ma[dd] += alpha * c.mv[dd]; }
+  for (int dd = c.lane; dd < nv; dd += 32) { c.qacc[dd] += alpha * c.search[dd]; c.Ma[dd] += alpha * c.mv[dd]; }
 #pragma unroll 1
-  for (int r = c.lane; r < c.nefc; r += NT) c.Jaref[r] += alpha * c.jv[r];
+  for (int r = c.lane; r < c.nefc; r += 32) c.Jaref[r] += alpha * c.jv[r];
   c.improvement = improvement;
-  tsync<NW>();
+  __syncwarp();
   return ls_converged;
 }
 
@@ -618,22 +540,16 @@ __device__ __forceinline__ void cg_direction(Ctx& c, const ModelDev& m, const Da
 // already drop an SM from 16 to 12 resident worlds -- measured 206 -> 250 us on the humanoid)
 // PLAIN: the model can produce neither equality nor friction-loss rows (no equalities, no dof / tendon frictionloss), so every row is
 // an inequality: ne = nf = 0 become compile-time constants and the two other row kinds drop out of the line search and the row pass
-template <bool ELL, bool BIG, bool CG, int NW, bool PLAIN = false, int NREG = 0>
-__global__ void __launch_bounds__(NW * 32, (NW == 1 && !BIG) ? 16 : 1)
+template <bool ELL, bool BIG, bool CG, bool PLAIN = false, int NREG = 0>
+__global__ void __launch_bounds__(32, BIG ? 1 : 16)
 k_solver(const __grid_constant__ ModelDev m, const __grid_constant__ DataDev d) {
   extern __shared__ float smem[];
-  constexpr int NT = 32 * NW;
-  const int lane = threadIdx.x;  // index inside the team of NW warps (one block) that owns the world
-  int w = blockIdx.x + d.w0;
-  if (d.rowcap > 0) {  // row-capacity class launch: the block's world comes from the class list
-    if ((int)blockIdx.x >= d.sol_count[2 * d.split_id + d.sol_class]) return;
-    w = d.sol_list[(size_t)d.sol_class * d.nworld + d.w0 + blockIdx.x];
-  }
+  const int lane = threadIdx.x;  // one warp (one block) owns the world
+  const int w = blockIdx.x + d.w0;
   if (w >= d.nworld) return;
   const SolLayout L = sol_layout(m, d, BIG);
   float* S = smem;
   const int nv = m.nv, njmax = d.njmax, nvp = d.nv_pad;
-  const int cap = sol_rowcap(d);  // rows of this world's shared-memory slice (njmax, or the row-capacity class of this launch)
   const size_t wb = (size_t)w;
   Ctx c;
   c.factored = false; c.chol_inv = 1.0f; c.chol_off = 0;
@@ -644,85 +560,70 @@ k_solver(const __grid_constant__ ModelDev m, const __grid_constant__ DataDev d) 
   const int vp = L.nvp;
   c.qacc = v; c.Ma = v + vp; c.grad = v + 2 * vp; c.search = v + 3 * vp; c.mv = v + 4 * vp; c.x = c.mv; c.qfs = v + 5 * vp; c.qfc = v + 6 * vp;
   float* rf = S + L.rowf;
-  c.Jaref = rf; c.jv = rf + cap; c.hw = c.jv; c.D = rf + 2 * cap; c.force = rf + 3 * cap;
-  c.floss = (m.nfricdof + m.ntenfric) > 0 ? rf + 4 * cap : c.D;  // never interpreted when the world has no friction rows
+  c.Jaref = rf; c.jv = rf + njmax; c.hw = c.jv; c.D = rf + 2 * njmax; c.force = rf + 3 * njmax;
+  c.floss = (m.nfricdof + m.ntenfric) > 0 ? rf + 4 * njmax : c.D;  // never interpreted when the world has no friction rows
   int* ri = (int*)(S + L.rowi);
-  c.state = ri; c.hidx = ri + cap;
-  c.njmax = cap; c.ncone = 0;
-  c.jcap = L.jcap; c.Jg = d.efc_J + wb * (size_t)d.njmax_pad * nvp;
+  c.state = ri; c.hidx = ri + njmax;
+  c.njmax = njmax; c.ncone = 0;
+  c.Jg = d.efc_J + wb * (size_t)d.njmax_pad * nvp;
   c.cgv = S + L.cgv;
-  c.red = S + L.red;
-  c.rng = (int*)(S + L.env); c.fz = c.rng + cap;
+  c.rng = (int*)(S + L.env); c.fz = c.rng + njmax;
   // a single tree with a floating base has a dense envelope (every row reaches the root dofs): bookkeeping would only cost
   c.env = BIG && m.ntree > 1;
-  c.rfri = rf + L.nrowf * cap; c.quad = c.rfri + cap; c.rinfo = ri + 2 * cap;
+  c.rfri = rf + L.nrowf * njmax; c.quad = c.rfri + njmax; c.rinfo = ri + 2 * njmax;
 
   if (njmax == 0 || nv == 0) {
 #pragma unroll 1
-    for (int dd = lane; dd < nv; dd += NT) d.qacc[wb * nv + dd] = d.qacc_smooth[wb * nv + dd];
+    for (int dd = lane; dd < nv; dd += 32) d.qacc[wb * nv + dd] = d.qacc_smooth[wb * nv + dd];
     if (lane == 0) d.solver_niter[w] = 0;
     return;
   }
-  const int nefc = min(min(d.nefc[w], njmax), cap);
+  const int nefc = min(d.nefc[w], njmax);
   c.nefc = nefc; c.ne = PLAIN ? 0 : d.ne[w]; c.nf = PLAIN ? 0 : d.nf[w];
 
-  // ---- stage the world's problem in shared memory.  One warp per world (NW = 1): the Jacobian rows and the per-row vectors are
-  // contiguous, 16-byte aligned blocks of the world-major arrays, so one lane issues a bulk-async copy (cp.async.bulk, SASS UBLKCP)
-  // for each and the warp waits once on the mbarrier, after it has issued its own small loads -- instead of four dependent
-  // load -> store loops in a row.  aref lands in the Jaref slot and is folded in below.
+  // ---- stage the world's problem in shared memory.  The Jacobian rows and the per-row vectors are contiguous, 16-byte aligned
+  // blocks of the world-major arrays, so one lane issues a bulk-async copy (cp.async.bulk, SASS UBLKCP) for each and the warp waits
+  // once on the mbarrier, after it has issued its own small loads -- instead of four dependent load -> store loops in a row.  aref
+  // lands in the Jaref slot and is folded in below.  Big models stage no Jacobian rows (see sol_layout).
   Stager st;
-  const int n4 = (nefc + 3) & ~3, nrow = n4 <= cap ? n4 : nefc;  // whole float4s when the slice has room (the pad is never read)
-  if (NW == 1) {
-    st.init(reinterpret_cast<uint64_t*>(S + L.bar), lane);
-    st.load(c.J, d.efc_J + wb * (size_t)d.njmax_pad * nvp, min(nefc, L.jcap) * nvp);
-    st.load(c.D, d.efc_D + wb * d.njmax_pad, nrow);
-    st.load(c.Jaref, d.efc_aref + wb * njmax, nrow);
-    if ((m.nfricdof + m.ntenfric) > 0) st.load(c.floss, d.efc_frictionloss + wb * njmax, nrow);
-  }
-  {
-    if (NW != 1) {
-      const float4* Jg = reinterpret_cast<const float4*>(d.efc_J + wb * (size_t)d.njmax_pad * nvp);
-      float4* Js = reinterpret_cast<float4*>(c.J);
+  const int n4 = (nefc + 3) & ~3, nrow = n4 <= njmax ? n4 : nefc;  // whole float4s when the slice has room (the pad is never read)
+  st.init(reinterpret_cast<uint64_t*>(S + L.bar), lane);
+  if (!BIG) st.load(c.J, c.Jg, nefc * nvp);
+  st.load(c.D, d.efc_D + wb * d.njmax_pad, nrow);
+  st.load(c.Jaref, d.efc_aref + wb * njmax, nrow);
+  if ((m.nfricdof + m.ntenfric) > 0) st.load(c.floss, d.efc_frictionloss + wb * njmax, nrow);
+  for (int i = lane; i < 7 * vp; i += 32) v[i] = 0.f;  // zero padding of every per-dof vector
+  __syncwarp();
 #pragma unroll 1
-      for (int i = lane; i < min(nefc, L.jcap) * nvp / 4; i += NT) Js[i] = Jg[i];
-    }
-    for (int i = lane; i < 7 * vp; i += NT) v[i] = 0.f;  // zero padding of every per-dof vector
-    tsync<NW>();
-#pragma unroll 1
-    for (int r = lane; r < nefc; r += NT) {
-      if (NW != 1) {
-        c.D[r] = d.efc_D[wb * d.njmax_pad + r];
-        if ((m.nfricdof + m.ntenfric) > 0) c.floss[r] = d.efc_frictionloss[wb * njmax + r];
+  for (int r = lane; r < nefc; r += 32) {
+    c.state[r] = ST_SATISFIED;
+    if (ELL) {  // row -> (contact, component) map; a contact's rows are consecutive (k_constraint.cu)
+      int info = -1; float fr = 0.f;
+      if (d.efc_type[wb * njmax + r] == CNSTR_CONTACT_ELLIPTIC) {
+        const int cid = d.efc_id[wb * njmax + r], e0 = d.contact_efc_address[(size_t)cid * m.nmaxpyramid], dim = d.contact_dim[cid], j = r - e0;
+        info = (e0 < 0 || e0 + dim > nefc) ? -2 : ((dim << 4) | j);
+        fr = j == 0 ? d.contact_friction[5 * (size_t)cid] * m.impratio_invsqrt : d.contact_friction[5 * (size_t)cid + j - 1];
       }
-      c.state[r] = ST_SATISFIED;
-      if (ELL) {  // row -> (contact, component) map; a contact's rows are consecutive (k_constraint.cu)
-        int info = -1; float fr = 0.f;
-        if (d.efc_type[wb * njmax + r] == CNSTR_CONTACT_ELLIPTIC) {
-          const int cid = d.efc_id[wb * njmax + r], e0 = d.contact_efc_address[(size_t)cid * m.nmaxpyramid], dim = d.contact_dim[cid], j = r - e0;
-          info = (e0 < 0 || e0 + dim > nefc) ? -2 : ((dim << 4) | j);
-          fr = j == 0 ? d.contact_friction[5 * (size_t)cid] * m.impratio_invsqrt : d.contact_friction[5 * (size_t)cid + j - 1];
-        }
-        c.rinfo[r] = info; c.rfri[r] = fr;
-      }
+      c.rinfo[r] = info; c.rfri[r] = fr;
     }
-    if (BIG) tcopy<NW>(c.M, d.M + wb * m.nC, m.nC, lane);
-    tcopy<NW>(c.qfs, d.qfrc_smooth + wb * nv, nv, lane);
-    const float* start = (m.disableflags & DSBL_WARMSTART) ? d.qacc_smooth : d.qacc_warmstart;
-    tcopy<NW>(c.qacc, start + wb * nv, nv, lane);
-    const int hsz = nv * (nv + 1) / 2;
-#pragma unroll 1
-    for (int e = lane; e < hsz; e += NT) { c.H[e] = 0.f; if (!BIG) c.M[e] = 0.f; }
   }
-  tsync<NW>();
+  if (BIG) tcopy(c.M, d.M + wb * m.nC, m.nC, lane);
+  tcopy(c.qfs, d.qfrc_smooth + wb * nv, nv, lane);
+  const float* start = (m.disableflags & DSBL_WARMSTART) ? d.qacc_smooth : d.qacc_warmstart;
+  tcopy(c.qacc, start + wb * nv, nv, lane);
+  const int hsz = nv * (nv + 1) / 2;
+#pragma unroll 1
+  for (int e = lane; e < hsz; e += 32) { c.H[e] = 0.f; if (!BIG) c.M[e] = 0.f; }
+  __syncwarp();
   if (c.env) {
 #pragma unroll 1
-    for (int i = lane; i < nv; i += NT) c.fz[i] = i;
-    tsync<NW>();
+    for (int i = lane; i < nv; i += 32) c.fz[i] = i;
+    __syncwarp();
   }
   if (!BIG) {  // dense packed M from the CSR values in global memory; H = M
     const float* Mg = d.M + wb * m.nC;
 #pragma unroll 4
-    for (int e = lane; e < m.nC; e += NT) {
+    for (int e = lane; e < m.nC; e += 32) {
       const int r = m.M_entry_row[e], col = m.M_colind[e];
       const float v = Mg[e];
       c.M[(r * (r + 1)) / 2 + col] = v;
@@ -730,28 +631,28 @@ k_solver(const __grid_constant__ ModelDev m, const __grid_constant__ DataDev d) 
     }
   } else {
 #pragma unroll 1
-    for (int e = lane; e < m.nC; e += NT) {  // lower triangle of M
+    for (int e = lane; e < m.nC; e += 32) {  // lower triangle of M
       const int r = m.M_entry_row[e], col = m.M_colind[e];
       c.H[(r * (r + 1)) / 2 + col] = c.M[e];
       if (c.env) atomicMin(&c.fz[r], col);
     }
   }
-  if (NW == 1) st.load_wait();  // staged rows and per-row vectors have landed
+  st.load_wait();  // staged rows and per-row vectors have landed
   if (c.env) {
     // nonzero column range [lo, hi) of every Jacobian row; rows of one elliptic contact share the union of their ranges (the cone
     // Hessian mixes them); every dof inside a row's range gets that row's lo into its envelope (H = M + sum of w J_r J_r^T terms)
 #pragma unroll 1
-    for (int r = lane; r < nefc; r += NT) {
+    for (int r = lane; r < nefc; r += 32) {
       const float* Jr = jrow<BIG>(c, r);
       int lo = nv, hi = 0;
       for (int k = 0; k < nv; k++) if (Jr[k] != 0.f) { lo = min(lo, k); hi = k + 1; }
       if (hi == 0) lo = 0;
       c.rng[r] = lo | (hi << 16);
     }
-    tsync<NW>();
+    __syncwarp();
     if (ELL) {
 #pragma unroll 1
-      for (int r = lane; r < nefc; r += NT) {
+      for (int r = lane; r < nefc; r += 32) {
         const int info = c.rinfo[r];
         if (info < 0 || (info & 15) != 0) continue;
         const int dim = info >> 4;
@@ -760,20 +661,20 @@ k_solver(const __grid_constant__ ModelDev m, const __grid_constant__ DataDev d) 
         if (hi == 0) lo = 0;
         for (int j = 0; j < dim; j++) c.rng[r + j] = lo | (hi << 16);
       }
-      tsync<NW>();
+      __syncwarp();
     }
 #pragma unroll 1
-    for (int r = lane; r < nefc; r += NT) {
+    for (int r = lane; r < nefc; r += 32) {
       const int lo = c.rng[r] & 0xFFFF, hi = c.rng[r] >> 16;
       for (int i = lo; i < hi; i++) atomicMin(&c.fz[i], lo);
     }
   }
 #pragma unroll 1
-  for (int r = lane; r < nefc; r += NT) {  // Jaref = J qacc - aref
-    c.Jaref[r] = row_dot(jrow<BIG>(c, r), c.qacc, c.nvp) - (NW == 1 ? c.Jaref[r] : d.efc_aref[wb * njmax + r]);
+  for (int r = lane; r < nefc; r += 32) {  // Jaref = J qacc - aref
+    c.Jaref[r] = row_dot(jrow<BIG>(c, r), c.qacc, c.nvp) - c.Jaref[r];
   }
-  mul_m<NW, BIG>(c, c.qacc, c.Ma);
-  tsync<NW>();
+  mul_m<BIG>(c, c.qacc, c.Ma);
+  __syncwarp();
 
   // One call site per phase: iteration -1 is init_context (solver.py:3622), iterations >= 0 are _solver_iteration (:3526).
   // _solve_done's three criteria are OR-ed (:3483-3486), so when `improvement` or `gradient` already satisfies the
@@ -781,9 +682,9 @@ k_solver(const __grid_constant__ ModelDev m, const __grid_constant__ DataDev d) 
   const float scale = m.meaninertia * (float)nv;
   int niter = 0, ovf = 0;
   for (int it = -1;; it++) {
-    if (it >= 0 && !linesearch<ELL, BIG, NW>(c)) ovf |= OVF_LS_ITERATIONS;
-    const int nlist = update_constraint<ELL, BIG, NW>(c, it < 0);
-    update_grad<NW>(c);
+    if (it >= 0 && !linesearch<ELL, BIG>(c)) ovf |= OVF_LS_ITERATIONS;
+    const int nlist = update_constraint<ELL, BIG>(c, it < 0);
+    update_grad(c);
     if (it >= 0) {
       niter++;
       const float improvement = c.improvement / scale, gradient = sqrtf(c.grad_dot) / scale;
@@ -794,7 +695,7 @@ k_solver(const __grid_constant__ ModelDev m, const __grid_constant__ DataDev d) 
       cg_direction(c, m, d, wb, it < 0);
       continue;
     }
-    if (!CG) update_search<ELL, BIG, NW, NREG>(c, nlist);
+    if (!CG) update_search<ELL, BIG, NREG>(c, nlist);
     if (it >= 0) {
       if (0.5f * c.newton_decrement / scale < m.tolerance) break;
       if (niter == m.iterations) { ovf |= OVF_ITERATIONS; break; }
@@ -802,117 +703,45 @@ k_solver(const __grid_constant__ ModelDev m, const __grid_constant__ DataDev d) 
   }
 
   // ---- results
-  tcopy<NW>(d.qacc + wb * nv, c.qacc, nv, lane);
-  tcopy<NW>(d.efc_Ma + wb * nv, c.Ma, nv, lane);
-  tcopy<NW>(d.qfrc_constraint + wb * nv, c.qfc, nv, lane);
+  tcopy(d.qacc + wb * nv, c.qacc, nv, lane);
+  tcopy(d.efc_Ma + wb * nv, c.Ma, nv, lane);
+  tcopy(d.qfrc_constraint + wb * nv, c.qfc, nv, lane);
 #pragma unroll 1
-  for (int r = lane; r < nefc; r += NT) { d.efc_force[wb * njmax + r] = c.force[r]; d.efc_state[wb * d.njmax_pad + r] = c.state[r]; }
+  for (int r = lane; r < nefc; r += 32) { d.efc_force[wb * njmax + r] = c.force[r]; d.efc_state[wb * d.njmax_pad + r] = c.state[r]; }
   if (lane == 0) { d.solver_niter[w] = niter; if (ovf) d.overflow[w] |= ovf; }
-}
-
-// Row-capacity classes.  A world's shared-memory slice is dominated by its staged Jacobian, sized for njmax rows although most worlds
-// hold far fewer (benchmark humanoid: njmax 64, ~18 rows while it stands): worlds whose row count fits rowcap = njmax / 2 are listed
-// here and solved by a launch with the smaller slice -- more of them are resident per SM, which is what the latency-bound solver's
-// time hangs on -- the rest by a launch with the full slice.  Lists are filled with one warp-aggregated atomic per warp; the order
-// inside a list depends on scheduling, the per-world results do not.
-__global__ void __launch_bounds__(256)
-k_solver_classify(const __grid_constant__ DataDev d, int cap0) {
-  const int i = blockIdx.x * blockDim.x + threadIdx.x, lane = threadIdx.x & 31;
-  const bool in = i < d.wn && i + d.w0 < d.nworld;
-  const int w = i + d.w0;
-  const int cls = in ? (min(d.nefc[w], d.njmax) <= cap0 ? 0 : 1) : -1;
-  for (int c = 0; c < 2; c++) {
-    const unsigned bal = __ballot_sync(FULL_MASK, cls == c);
-    if (!bal) continue;
-    int base = 0;
-    if (lane == __ffs(bal) - 1) base = atomicAdd(&d.sol_count[2 * d.split_id + c], __popc(bal));
-    base = __shfl_sync(FULL_MASK, base, __ffs(bal) - 1);
-    if (cls == c) d.sol_list[(size_t)c * d.nworld + d.w0 + base + __popc(bal & ((1u << lane) - 1u))] = w;
-  }
 }
 
 }  // namespace
 
-// The "big" instantiation (packed Hessian and factor worked on in shared memory, Jacobian rows read through L2, CSR inertia) is mandatory
-// above nv = 32; MJB_SOLVER_BIG = 1 selects it for small models too (62 instead of 127 registers, 6.4 instead of 14 KB per world).
-static bool solver_big(const ModelDev& m) {
-  static int forced = -1;
-  if (forced < 0) { const char* e = getenv("MJB_SOLVER_BIG"); forced = e ? atoi(e) : 0; }
-  return m.nv > 32 || forced == 1;
-}
-size_t smem_solver(const ModelDev& m, const DataDev& d) { return (size_t)sol_layout(m, d, solver_big(m)).total * sizeof(float); }
+size_t smem_solver(const ModelDev& m, const DataDev& d) { return (size_t)sol_layout(m, d, m.nv > 32).total * sizeof(float); }
 
-// Warps per world: 1.  For nv > 32 the per-world slice of shared memory (packed Hessian + factor + Jacobian rows) limits an SM to
-// a few resident worlds; teams of 2 or 4 warps per world (block barriers, right-looking team Cholesky) are implemented and
-// parity-tested but measured slower than one warp per world, so they stay an experiment knob: MJB_SOLVER_WARPS = 1, 2 or 4.
-static int solver_warps(const ModelDev& m) {
-  if (m.nv <= 32 || m.solver == SOL_CG) return 1;
-  static int forced = -1;
-  if (forced < 0) { const char* e = getenv("MJB_SOLVER_WARPS"); forced = e ? atoi(e) : 0; }
-  if (forced == 1 || forced == 2 || forced == 4) return forced;
-  return 1;  // teams of 2 / 4 warps measured slower on unitree G1 and three_humanoids (block barriers per Cholesky column)
-}
-
-// row-capacity classes (see k_solver_classify): small-model path with a staged Jacobian, enough rows and worlds to matter
-static bool solver_uses_classes(const ModelDev& m, const DataDev& d) {
-  static int classes = -1;
-  // off by default: measured slower for the humanoid, with every world in the small class and with a mixed population -- the extra
-  // resident worlds do not speed the solve up, so its time is not set by the number of worlds in
-  // flight the way the position / velocity kernels' is; kept as an experiment knob (MJB_SOLVER_CLASSES=1), parity-tested
-  if (classes < 0) { const char* e = getenv("MJB_SOLVER_CLASSES"); classes = e ? atoi(e) : 0; }
-  return classes && !solver_big(m) && d.rowcap == 0 && d.njmax >= 32 && d.wn >= 256 && d.sol_list;
-}
-int solver_launch_count(const ModelDev& m, const DataDev& d) { return solver_uses_classes(m, d) ? 3 : 1; }
-
+// One warp per world.  The "big" instantiation (packed Hessian and factor worked on in shared memory, Jacobian rows read through L2,
+// CSR inertia) is the path above nv = 32.
 cudaError_t launch_solver(const ModelDev& m, const DataDev& d, cudaStream_t s) {
   const size_t smem = smem_solver(m, d);
-  const int ell = m.cone == CONE_ELLIPTIC ? 1 : 0, big = solver_big(m) ? 1 : 0, cg = m.solver == SOL_CG ? 1 : 0;
-  const int nw = solver_warps(m), team = nw == 4 ? 2 : (nw == 2 ? 1 : 0);
-  const int which = cg ? 4 + 2 * big + ell : (big ? 8 + 2 * team + ell : ell);
-  static size_t configured[18] = {0};
-  static void (*const kerns[14])(ModelDev, DataDev) = {
-    k_solver<false, false, false, 1>, k_solver<true, false, false, 1>, nullptr, nullptr,
-    k_solver<false, false, true, 1>,  k_solver<true, false, true, 1>,  k_solver<false, true, true, 1>,  k_solver<true, true, true, 1>,
-    k_solver<false, true, false, 1>,  k_solver<true, true, false, 1>,  k_solver<false, true, false, 2>, k_solver<true, true, false, 2>,
-    k_solver<false, true, false, 4>,  k_solver<true, true, false, 4>};
+  const int ell = m.cone == CONE_ELLIPTIC ? 1 : 0, big = m.nv > 32 ? 1 : 0, cg = m.solver == SOL_CG ? 1 : 0;
+  const int which = 4 * cg + 2 * big + ell;
+  static size_t configured[12] = {0};
+  static void (*const kerns[8])(ModelDev, DataDev) = {
+    k_solver<false, false, false>, k_solver<true, false, false>, k_solver<false, true, false>, k_solver<true, true, false>,
+    k_solver<false, false, true>,  k_solver<true, false, true>,  k_solver<false, true, true>,  k_solver<true, true, true>};
   void (*kern)(ModelDev, DataDev) = kerns[which];
   int ci = which;
   // no equality and no friction-loss rows possible: the instantiation with ne = nf = 0 compiled in (humanoid solver 202 -> 181 us: the
   // line-search loops lose two of their three row kinds, and with them instructions and instruction-cache footprint)
   const bool plain = m.neq == 0 && m.nfricdof == 0 && m.ntenfric == 0 && m.ntendon == 0;
   if (which == 0 && plain) {
-    kern = k_solver<false, false, false, 1, true>; ci = 14;
+    kern = k_solver<false, false, false, true>; ci = 8;
     // ... and the register-row size fixed (one Hessian / Cholesky variant in the kernel instead of five: 182 -> 178 us)
-    if (m.nv > 24 && m.nv <= 28 && d.nv_pad == 28) { kern = k_solver<false, false, false, 1, true, 28>; ci = 15; }
-    else if (m.nv > 28 && d.nv_pad == 32) { kern = k_solver<false, false, false, 1, true, 32>; ci = 16; }
+    if (m.nv > 24 && m.nv <= 28 && d.nv_pad == 28) { kern = k_solver<false, false, false, true, 28>; ci = 9; }
+    else if (m.nv > 28 && d.nv_pad == 32) { kern = k_solver<false, false, false, true, 32>; ci = 10; }
   }
-  if (which == 8 && plain) { kern = k_solver<false, true, false, 1, true>; ci = 17; }  // nv > 32 (unitree G1, three_humanoids)
+  if (which == 2 && plain) { kern = k_solver<false, true, false, true>; ci = 11; }  // nv > 32 (unitree G1, three_humanoids)
   if (smem > 48 * 1024 && smem > configured[ci]) {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     configured[ci] = smem;
   }
-  const int cap0 = ((d.njmax / 2) + 3) & ~3;
-  if (solver_uses_classes(m, d)) {
-    cudaError_t e = cudaMemsetAsync(d.sol_count + 2 * d.split_id, 0, 2 * sizeof(int), s);
-    if (e != cudaSuccess) return e;
-    k_solver_classify<<<(d.wn + 255) / 256, 256, 0, s>>>(d, cap0);
-    // the two classes run concurrently (fork / join on the range's auxiliary stream): with different slice sizes they cannot share a
-    // launch, and back to back each would pay its own last, partly empty round of resident blocks
-    cudaStream_t aux = (cudaStream_t)d.sol_stream;
-    cudaEvent_t fork = (cudaEvent_t)d.sol_fork, join = (cudaEvent_t)d.sol_join;
-    if ((e = cudaEventRecord(fork, s)) != cudaSuccess) return e;
-    if ((e = cudaStreamWaitEvent(aux, fork, 0)) != cudaSuccess) return e;
-    DataDev dc = d;
-    dc.rowcap = d.njmax; dc.sol_class = 1;
-    kern<<<d.wn, nw * 32, smem, aux>>>(m, dc);  // blocks beyond the class count exit at once
-    if ((e = cudaEventRecord(join, aux)) != cudaSuccess) return e;
-    dc.rowcap = cap0; dc.sol_class = 0;
-    kern<<<d.wn, nw * 32, smem_solver(m, dc), s>>>(m, dc);
-    if ((e = cudaStreamWaitEvent(s, join, 0)) != cudaSuccess) return e;
-    return cudaGetLastError();
-  }
-  const int grid = d.wn;
-  kern<<<grid, nw * 32, smem, s>>>(m, d);
+  kern<<<d.wn, 32, smem, s>>>(m, d);
   return cudaGetLastError();
 }

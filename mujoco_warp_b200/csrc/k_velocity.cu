@@ -10,7 +10,6 @@
 // bulk-async (TMA) copies of the contiguous [G][n] blocks.  Tree passes are level-synchronous in shared memory, children
 // are gathered by the parent in a fixed order (no float atomics => bit-reproducible), the inertia blocks are factored by the
 // team in shared memory directly in the qLD layout (upper factor, row-major), so qLD leaves as one bulk store.
-#include <cstdlib>
 
 #include "mjb_math.cuh"
 #include "mjb_team.cuh"
@@ -164,7 +163,6 @@ k_velocity(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
     // com_vel: level-synchronous forward pass
     if (v_all || (mask & STG_COMVEL)) {
     if (sub < 6) cvel[sub] = 0.f;
-    if (LPW < 6 && sub == 0) { cvel[4] = 0.f; cvel[5] = 0.f; }
     __syncwarp();
 #pragma unroll 1
     for (int l = 1; l < m.nlevel; l++) {
@@ -494,7 +492,7 @@ k_velocity(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
 template <bool PEXT>
 static void (*vel_kernel(int lpw, bool bat))(ModelDev, DataDev, int) {
   if (bat) return k_velocity<PEXT, 32, true>;
-  return lpw == 4 ? k_velocity<PEXT, 4, false> : lpw == 8 ? k_velocity<PEXT, 8, false> : lpw == 16 ? k_velocity<PEXT, 16, false> : k_velocity<PEXT, 32, false>;
+  return lpw == 8 ? k_velocity<PEXT, 8, false> : lpw == 16 ? k_velocity<PEXT, 16, false> : k_velocity<PEXT, 32, false>;
 }
 // has_gravcomp also flags free / ball joint springs (io.py put_model); tendons live in the same instantiation
 static bool vel_ext(const ModelDev& m) { return m.has_gravcomp || m.ntendon > 0; }
@@ -503,7 +501,7 @@ static void (*vel_kernel(const ModelDev& m, int lpw))(ModelDev, DataDev, int) {
 }
 
 static TeamShape vel_shape(const ModelDev& m, const DataDev& d) {
-  TeamShape t = team_shape((size_t)vel_layout(m).total, d.wn, "MJB_LPW_VEL", "MJB_WPB_VEL", [&](int lpw) { return kernel_regs(vel_kernel(m, lpw)); });
+  TeamShape t = team_shape((size_t)vel_layout(m).total, d.wn, [&](int lpw) { return kernel_regs(vel_kernel(m, lpw)); });
   if (m.batched && t.lpw != 32) t = team_shape_fixed((size_t)vel_layout(m).total, 32, 2);
   return t;
 }
@@ -511,8 +509,8 @@ size_t smem_velocity(const ModelDev& m, const DataDev& d) { return vel_shape(m, 
 
 // the kernel instance for the launch shape, configured on its first use
 static cudaError_t vel_configured(const ModelDev& m, const TeamShape& t, void (**kern)(ModelDev, DataDev, int)) {
-  static TeamConfig configured[2][5];
-  const int ext = vel_ext(m) ? 1 : 0, ki = m.batched ? 4 : t.lpw == 4 ? 0 : t.lpw == 8 ? 1 : t.lpw == 16 ? 2 : 3;
+  static TeamConfig configured[2][4];
+  const int ext = vel_ext(m) ? 1 : 0, ki = m.batched ? 3 : t.lpw == 8 ? 0 : t.lpw == 16 ? 1 : 2;
   *kern = vel_kernel(m, t.lpw);
   return team_configure(*kern, t.block_bytes, &configured[ext][ki]);
 }

@@ -129,51 +129,6 @@ __device__ __forceinline__ void warp_chol_solve_packed_env(const float* L, int n
   }
 }
 
-// Team (NW warps = one block) variants of the packed factor / solve for the multi-warp solver: right-looking, so that the
-// O(n^2) trailing update of every column is spread over all 32 NW threads (entry (a, b) of the trailing triangle is decoded
-// from a flat index); three block barriers per column.
-template <int NW>
-__device__ __forceinline__ void team_cholesky_packed(float* A, int n, int tid) {
-  constexpr int NT = 32 * NW;
-  for (int j = 0; j < n; j++) {
-    const int jj = (j * (j + 1)) / 2 + j;
-    if (tid == 0) A[jj] = sqrtf(fmaxf(A[jj], MJ_MINVAL));
-    __syncthreads();
-    const float inv = 1.0f / A[jj];
-    for (int i = j + 1 + tid; i < n; i += NT) A[(i * (i + 1)) / 2 + j] *= inv;
-    __syncthreads();
-    const int mrem = n - 1 - j, cnt = mrem * (mrem + 1) / 2;
-    for (int e = tid; e < cnt; e += NT) {
-      int a = (int)((sqrtf(8.0f * (float)e + 1.0f) - 1.0f) * 0.5f);
-      while ((a + 1) * (a + 2) / 2 <= e) a++;
-      while (a * (a + 1) / 2 > e) a--;
-      const int b = e - a * (a + 1) / 2, i = j + 1 + a, k = j + 1 + b;
-      const int ri = (i * (i + 1)) / 2;
-      A[ri + k] -= A[ri + j] * A[(k * (k + 1)) / 2 + j];
-    }
-    __syncthreads();
-  }
-}
-template <int NW>
-__device__ __forceinline__ void team_chol_solve_packed(const float* L, int n, float* x, int tid) {
-  constexpr int NT = 32 * NW;
-  for (int j = 0; j < n; j++) {  // forward: L y = b
-    const float yj = x[j] / L[(j * (j + 1)) / 2 + j];
-    __syncthreads();
-    for (int i = j + 1 + tid; i < n; i += NT) x[i] -= L[(i * (i + 1)) / 2 + j] * yj;
-    if (tid == 0) x[j] = yj;
-    __syncthreads();
-  }
-  for (int j = n - 1; j >= 0; j--) {  // backward: L^T x = y
-    const float* rj = L + (j * (j + 1)) / 2;
-    const float xj = x[j] / rj[j];
-    __syncthreads();
-    for (int i = tid; i < j; i += NT) x[i] -= rj[i] * xj;
-    if (tid == 0) x[j] = xj;
-    __syncthreads();
-  }
-}
-
 // ------------------------------------------------------------------------------------------------------------------
 // Register-resident Cholesky for n <= 32: lane i keeps row i of the matrix in registers, columns are eliminated
 // right-looking with warp shuffles (no shared-memory round trips, no __syncwarp per column), the forward substitution of
@@ -236,51 +191,6 @@ __device__ __forceinline__ float chol_solve_rows(float (&a)[N], int n, float b, 
   return b;
 }
 
-// Same factor + solve with a ROLLED column loop: after eliminating a column every lane rotates its row registers by one
-// (a[k-1] <- a[k] - l_ij * l_kj), so the pivot column always sits in a[0] and the loop body is identical for every column.
-// Executes ~n*N instead of ~N^2/2 SHFL/FFMA pairs but is ~25x smaller: the fully unrolled sweep (30 KB of SASS for N = 28)
-// thrashed the instruction cache (ncu: `no_instruction` was the top stall of k_solver).
-template <int N, bool PACKED = false>
-__device__ __forceinline__ float chol_solve_rows_rolled(float (&a)[N], int n, float b, float* Ls, int ldL, int lane) {
-  float myinv = 1.0f;
-#pragma unroll 1
-  for (int j = 0; j < n; j++) {
-    const float ajj = __shfl_sync(FULL_MASK, a[0], j);
-    const float inv = rsqrtf(fmaxf(ajj, MJ_MINVAL));
-    const float lij = a[0] * inv;  // column j of L (meaningful for lanes >= j)
-    if (lane == j) myinv = inv;
-    const float yj = __shfl_sync(FULL_MASK, b, j) * inv;
-    b = lane > j ? b - lij * yj : (lane == j ? yj : b);
-    if (lane >= j && lane < n) Ls[tri_at<PACKED>(lane, j, ldL)] = lij;
-    // trailing update of the n-1-j columns to the right, in chunks of 4 with a warp-uniform early exit (registers past the
-    // matrix edge are never read again, so they need not be shifted); srcLane >= 32 wraps modulo 32 by definition of SHFL
-    const int rem = n - 1 - j;
-#pragma unroll
-    for (int k0 = 1; k0 < N; k0 += 4) {
-      if (k0 > rem) break;
-#pragma unroll
-      for (int kk = 0; kk < 4; kk++) {
-        const int k = k0 + kk;
-        if (k < N) {
-          const float lkj = __shfl_sync(FULL_MASK, lij, j + k);
-          a[k - 1] = a[k] - lij * lkj;
-        }
-      }
-    }
-  }
-  __syncwarp();
-#pragma unroll 1
-  for (int j = n - 1; j >= 0; j--) {
-    const float xj = __shfl_sync(FULL_MASK, b * myinv, j);
-    const float ltj = lane < j ? Ls[tri_at<PACKED>(j, lane, ldL)] : 0.f;
-    b = lane < j ? b - ltj * xj : (lane == j ? xj : b);
-  }
-  return b;
-}
-
-// Column-major storage of the factor's sub-diagonal part for the broadcast variant below: column j keeps its c = n - 1 - j
-// entries L[j+1 .. n-1][j] contiguously, padded to a multiple of 4 floats, columns ordered by increasing c, so that every
-// column starts 16-byte aligned.  colsub_off(c) = sum_{t < c} pad4(t); the whole factor takes colsub_off(n) floats (420 for n = 28).
 // 1 / sqrt(x) for x known to be a normal number (callers clamp at MJ_MINVAL): the bare MUFU.RSQ, without the denormal rescaling
 // rsqrtf() wraps around it -- same bits for normal inputs.
 __device__ __forceinline__ float rsqrt_normal(float x) {
@@ -289,89 +199,11 @@ __device__ __forceinline__ float rsqrt_normal(float x) {
   return y;
 }
 
-__host__ __device__ __forceinline__ int colsub_off(int c) {
-  if (c <= 0) return 0;
-  const int U = (c - 1) >> 2;
-  return 8 * U * (U + 1) + 4 * (U + 1) * (c - 1 - 4 * U);
-}
-
-// Factor + solve with the rolled column loop as above, but the pivot column is broadcast through shared memory instead of
-// one SHFL per trailing column: every lane stores its l_ij into the column's (16-byte aligned) slot, then all lanes read
-// four multipliers per LDS.128 (same address in every lane: a broadcast, one wavefront).  ncu on the humanoid: the SHFL
-// sweep was 44 % of the solver's instructions (30 % of those the SHFL + lane arithmetic, 16 % the FMA); this version issues
-// a quarter of the data-movement instructions and leaves the SHFL pipe to the two per-column broadcasts.
-//   a[]  : row `lane` of the matrix (consumed);  Lc : colsub_off(n) floats of scratch, receives the factor (layout above)
-template <int N>
-__device__ __forceinline__ float chol_solve_rows_bcast(float (&a)[N], int n, float b, float* Lc, int lane, float& myinv) {
-  myinv = 1.0f;
-  int coff = colsub_off(n - 1);      // slot offset of column j (rem = n - 1 - j entries), updated incrementally
-  float* lanecol = Lc + lane - 1;    // lane's slot in column j is lanecol[coff - j]
-  const bool row = lane < n;
-#pragma unroll 1
-  for (int j = 0; j < n; j++) {
-    const float ajj = __shfl_sync(FULL_MASK, a[0], j);
-    const float inv = rsqrt_normal(fmaxf(ajj, MJ_MINVAL));
-    const float lij = a[0] * inv;  // column j of L (meaningful for lanes >= j)
-    if (lane == j) myinv = inv;
-    // forward substitution folded in: lanes below the pivot subtract l_ij y_j; the pivot lane keeps its unscaled b (y_j = b * myinv)
-    const float yj = __shfl_sync(FULL_MASK, b, j) * inv;
-    b -= lane > j ? lij * yj : 0.f;
-    const int rem = n - 1 - j;
-    const float* col = Lc + coff;
-    if (lane > j && row) lanecol[coff - j] = lij;
-    __syncwarp();
-    // trailing update of the rem columns to the right; registers are rotated by one so the next pivot sits in a[0]
-#pragma unroll
-    for (int k0 = 1; k0 < N; k0 += 4) {
-      if (k0 > rem) break;
-      const float4 l = *reinterpret_cast<const float4*>(col + (k0 - 1));
-      a[k0 - 1] = a[k0] - lij * l.x;
-      if (k0 + 1 < N) a[k0] = a[k0 + 1] - lij * l.y;
-      if (k0 + 2 < N) a[k0 + 1] = a[k0 + 2] - lij * l.z;
-      if (k0 + 3 < N) a[k0 + 2] = a[k0 + 3] - lij * l.w;
-    }
-    coff -= (rem + 2) & ~3;  // colsub_off(rem) - colsub_off(rem - 1) = pad4(rem - 1)
-  }
-  // backward substitution: L[j][lane] for lane < j sits in column `lane`, slot j - lane - 1
-  const float* mycol = Lc + colsub_off(n - 1 - lane) - lane - 1;
-  b *= myinv;  // y
-#pragma unroll 1
-  for (int j = n - 1; j >= 0; j--) {  // x_j = (y_j - sum_{i > j} L_ij x_i) / L_jj; lane i < j accumulates -L_ji x_j, lanes >= j hold ltj = 0
-    const float xj = __shfl_sync(FULL_MASK, b * myinv, j);
-    const float ltj = lane < j ? mycol[j] : 0.f;
-    b -= ltj * xj;
-  }
-  return b * myinv;
-}
-
-// Solve only, with the factor chol_solve_rows_bcast left in Lc and the reciprocal diagonal it returned in myinv (lane j holds
-// 1 / L_jj): the same operations in the same order as the substitutions folded into the factorisation, so the result is
-// bit-identical to factoring the same matrix again.
-__device__ __forceinline__ float chol_subst_bcast(int n, float b, const float* Lc, int lane, float myinv) {
-  int coff = colsub_off(n - 1);
-  const float* lanecol = Lc + lane - 1;
-  const bool row = lane < n;
-#pragma unroll 1
-  for (int j = 0; j < n; j++) {
-    const float yj = __shfl_sync(FULL_MASK, b * myinv, j);
-    const float lij = (lane > j && row) ? lanecol[coff - j] : 0.f;
-    b -= lane > j ? lij * yj : 0.f;
-    coff -= (n - j + 1) & ~3;  // (rem + 2) & ~3 with rem = n - 1 - j
-  }
-  const float* mycol = Lc + colsub_off(n - 1 - lane) - lane - 1;
-  b *= myinv;
-#pragma unroll 1
-  for (int j = n - 1; j >= 0; j--) {
-    const float xj = __shfl_sync(FULL_MASK, b * myinv, j);
-    const float ltj = lane < j ? mycol[j] : 0.f;
-    b -= ltj * xj;
-  }
-  return b * myinv;
-}
-
-// ---- Two columns per sweep.  The per-column bookkeeping of chol_solve_rows_bcast (pivot broadcast, reciprocal square root, slot
-// arithmetic, barrier, loop control: about half of its ~90 instructions per column) is paid once per PAIR of columns here, and a row
-// makes one shared-memory round trip per pair instead of one per column.  Columns (j, j+1) are eliminated together:
+// ---- Factor + solve for n <= 32 with a rolled loop over PAIRS of columns: lane i holds row i in registers, which rotate by two
+// after each pair so the next pivots always sit in a[0], a[1].  The per-column bookkeeping (pivot broadcast, reciprocal square root,
+// slot arithmetic, barrier, loop control) is paid once per pair, and a row makes one shared-memory round trip per pair.  The pair's
+// two factor columns are broadcast to every lane through shared memory (LDS.128 of the same address).  A rolled loop keeps the
+// sweep small enough for the instruction cache.  Columns (j, j+1) are eliminated together:
 //   l0 = a[0] / sqrt(a00);  l10 = l0 of row j+1;  t1 = a[1] - l0 l10;  l1 = t1 / sqrt(t1 of row j+1)
 //   a[k-2] <- a[k] - l0 L[j+k][j] - l1 L[j+k][j+1]     (registers rotate by two)
 // Storage of the factor, per pair p (columns 2p, 2p+1, cnt = ne - 2p - 2 rows below the pair, ne = n rounded up to even):
@@ -467,54 +299,6 @@ __device__ __forceinline__ float chol_subst_pair(int n, float b, const float* Lc
     b -= ltj * xj;
   }
   return b * myinv;
-}
-
-// The same factor + solve with the column loop fully unrolled: row registers are addressed statically (no rotation), column slots and
-// chunk counts are compile-time, the per-column bookkeeping of the rolled loop (offsets, trip counts, register moves: ~40 of its ~65
-// instructions per column) disappears.  ~1000 instructions for N = 28 instead of ~2300 -- and yet measured SLOWER (150 registers):
-// every warp streams ~16 KB of straight-line code per factorisation through the instruction
-// cache.  Kept behind MJB_CHOL_UNROLLED for reference; the rolled loop above is what ships.  Lc holds colsub_off(N) floats,
-// laid out for the padded size N (rows >= n are identity padding and produce zero multipliers).
-template <int N>
-__device__ __forceinline__ float chol_solve_rows_unrolled(float (&a)[N], int n, float b, float* Lc, int lane) {
-  float myinv = 1.0f;
-  float* lanecol = Lc + lane - 1;  // lane's slot in column j is lanecol[colsub_off(N - 1 - j) - j]
-#pragma unroll
-  for (int j = 0; j < N; j++) {
-    if (j < n) {
-      const float ajj = __shfl_sync(FULL_MASK, a[j], j);
-      const float inv = rsqrtf(fmaxf(ajj, MJ_MINVAL));
-      const float lij = a[j] * inv;  // column j of L (meaningful for lanes >= j)
-      if (lane == j) myinv = inv;
-      const float yj = __shfl_sync(FULL_MASK, b, j) * inv;
-      b = lane > j ? b - lij * yj : (lane == j ? yj : b);
-      if (j + 1 < N) {
-        constexpr int dummy = 0; (void)dummy;
-        float* col = Lc + colsub_off(N - 1 - j);
-        if (lane > j && lane < N) lanecol[colsub_off(N - 1 - j) - j] = lij;
-        __syncwarp();
-#pragma unroll
-        for (int k0 = j + 1; k0 < N; k0 += 4) {
-          const float4 l = *reinterpret_cast<const float4*>(col + (k0 - j - 1));
-          a[k0] -= lij * l.x;
-          if (k0 + 1 < N) a[k0 + 1] -= lij * l.y;
-          if (k0 + 2 < N) a[k0 + 2] -= lij * l.z;
-          if (k0 + 3 < N) a[k0 + 3] -= lij * l.w;
-        }
-      }
-    }
-  }
-  // backward substitution: L[j][lane] for lane < j sits in column `lane`, slot j - lane - 1
-  const float* mycol = Lc + colsub_off(N - 1 - lane) - lane - 1;
-#pragma unroll
-  for (int j = N - 1; j >= 0; j--) {
-    if (j < n) {
-      const float xj = __shfl_sync(FULL_MASK, b * myinv, j);
-      const float ltj = lane < j ? mycol[j] : 0.f;
-      b = lane < j ? b - ltj * xj : (lane == j ? xj : b);
-    }
-  }
-  return b;
 }
 
 template <int N>

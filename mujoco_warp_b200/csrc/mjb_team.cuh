@@ -13,7 +13,6 @@
 #include <algorithm>
 #include <climits>
 #include <cstdint>
-#include <cstdlib>
 #include <cuda_runtime.h>
 
 #include "mjb_math.cuh"
@@ -165,36 +164,27 @@ inline cudaError_t team_configure(K* kern, size_t smem, TeamConfig* c) {
 // The team kernels are latency bound, so their time is the number of residency rounds (waves of blocks that fit on the SMs at
 // once) times one warp's dependent chain (DESIGN.md §3).  The warps per block (1, 2 or 4) are those that need the fewest rounds
 // for `nworld` worlds, with as many blocks per SM as its shared memory, register file (`regs_of(lpw)`: registers per thread of
-// the kernel instance for lpw), block and warp limits allow; ties go to two-warp blocks.  MJB_LPW_* / MJB_WPB_* override.
+// the kernel instance for lpw), block and warp limits allow; ties go to two-warp blocks.
 struct TeamShape { int lpw, wpb; size_t warp_bytes, block_bytes; };
 template <class F>
-inline TeamShape team_shape(size_t world_words, int nworld, const char* env_lpw, const char* env_wpb, F regs_of) {
+inline TeamShape team_shape(size_t world_words, int nworld, F regs_of) {
   constexpr size_t kBlockMax = 200 * 1024;  // leaves room for a second resident block's reserve
   auto bytes = [&](int lpw) { return (world_words * (size_t)(32 / lpw) + 4) * sizeof(float); };
-  const char* e = getenv(env_lpw);
-  int lpw = e ? atoi(e) : 8;
-  if (lpw != 4 && lpw != 8 && lpw != 16 && lpw != 32) lpw = 8;
+  int lpw = 8;
   while (lpw < 32 && bytes(lpw) > kBlockMax / 2) lpw *= 2;
-  e = getenv(env_wpb);
   int wpb = 2;
-  if (e) {
-    wpb = atoi(e);
-  } else {
-    const SmLimits& sm = sm_limits();
-    const long groups = (nworld + 32 / lpw - 1) / (32 / lpw);
-    const int warp_regs = (regs_of(lpw) * 32 + 255) & ~255;  // registers are allocated per warp in units of 256
-    auto rounds = [&](int w) {
-      long per_sm = (long)(sm.smem_per_sm / sm_block_bytes(bytes(lpw) * w));
-      per_sm = std::min({per_sm, (long)sm.blocks, (long)(sm.warps / w)});
-      if (warp_regs > 0) per_sm = std::min(per_sm, (long)(sm.regs / warp_regs / w));
-      const long fit = per_sm * sm.sms, blocks = (groups + w - 1) / w;  // fit: blocks resident at once
-      return fit > 0 ? (blocks + fit - 1) / fit : LONG_MAX;
-    };
-    for (int w : {1, 4})
-      if (bytes(lpw) * w <= kBlockMax && rounds(w) < rounds(wpb)) wpb = w;
-  }
-  if (wpb < 1) wpb = 1;
-  if (wpb > 8) wpb = 8;
+  const SmLimits& sm = sm_limits();
+  const long groups = (nworld + 32 / lpw - 1) / (32 / lpw);
+  const int warp_regs = (regs_of(lpw) * 32 + 255) & ~255;  // registers are allocated per warp in units of 256
+  auto rounds = [&](int w) {
+    long per_sm = (long)(sm.smem_per_sm / sm_block_bytes(bytes(lpw) * w));
+    per_sm = std::min({per_sm, (long)sm.blocks, (long)(sm.warps / w)});
+    if (warp_regs > 0) per_sm = std::min(per_sm, (long)(sm.regs / warp_regs / w));
+    const long fit = per_sm * sm.sms, blocks = (groups + w - 1) / w;  // fit: blocks resident at once
+    return fit > 0 ? (blocks + fit - 1) / fit : LONG_MAX;
+  };
+  for (int w : {1, 4})
+    if (bytes(lpw) * w <= kBlockMax && rounds(w) < rounds(wpb)) wpb = w;
   while (wpb > 1 && bytes(lpw) * wpb > kBlockMax) wpb--;
   TeamShape t;
   t.lpw = lpw; t.wpb = wpb; t.warp_bytes = bytes(lpw); t.block_bytes = t.warp_bytes * wpb;

@@ -98,7 +98,6 @@ struct DataDev {
   int nworld, nconmax, naconmax, njmax, njmax_pad, nv_pad;
   int w0, wn;  // world range [w0, w0 + wn) processed by one launch (the step is pipelined over two world halves)
   int njmax_nnz;  // capacity of the CSR view of efc.J (0: dense model, no CSR view)
-  int jcap;    // nv > 32: Jacobian rows the solver stages in shared memory (the rest is read from global memory / L2)
 #define X(n) float* __restrict__ n;
   MJB_DATA_FARRS(X)
 #undef X
@@ -109,15 +108,6 @@ struct DataDev {
   int* world_conadr;  // (nworld) first contact-pool slot of each world's contiguous block
   int* world_ncon;    // (nworld) number of contacts the world wrote this step
   float* imp_qacc;    // (nworld, nv) acceleration solved by the fully implicit integrator (k_implicit.cu), consumed by the advance kernel
-  // solver row-capacity classes (k_solver.cu): worlds whose constraint count fits rowcap rows run with a smaller shared-memory slice
-  int* sol_list;      // (2, nworld) world ids per class, each launch range [w0, w0 + wn) owns that sub-range of both rows
-  int* sol_count;     // (8, 2) worlds per (split, class)
-  int split_id;       // which of the pipelined world ranges this launch covers
-  int rowcap;         // > 0: the solver launch stages at most this many rows per world and takes its worlds from sol_list[sol_class]
-  int sol_class;
-  // host-side handles of this launch range (opaque to kernels): auxiliary stream + fork / join events on which the second
-  // row-capacity class of the solver runs concurrently with the first
-  void *sol_stream, *sol_fork, *sol_join;
 };
 
 // ---------------------------------------------------------------- enums (MuJoCo values; see constants.py)
@@ -176,7 +166,6 @@ cudaError_t launch_velocity(const ModelDev& m, const DataDev& d, int stage_mask,
 cudaError_t launch_solve_m(const ModelDev& m, const DataDev& d, float* x, const float* y, cudaStream_t s);
 cudaError_t launch_mul_m(const ModelDev& m, const DataDev& d, float* res, const float* vec, cudaStream_t s);
 cudaError_t launch_solver(const ModelDev& m, const DataDev& d, cudaStream_t s);
-int solver_launch_count(const ModelDev& m, const DataDev& d);  // kernels launch_solver issues (row-capacity classes: classify + two solves)
 cudaError_t launch_integrate(const ModelDev& m, const DataDev& d, int integrator, cudaStream_t s);
 cudaError_t launch_implicit_solve(const ModelDev& m, const DataDev& d, float* qacc_out, cudaStream_t s);  // fully implicit integrator: qLU and its solve
 size_t smem_implicit(const ModelDev& m);

@@ -161,17 +161,16 @@ def test_world_split_pipeline_is_bit_identical(built, scene, tmp_path):
   script.write_text(SPLIT_SCRIPT)
   nworld = 2048
   outs = {}
-  # the third knob is MJB_FORK: k_velocity on its own stream next to k_collision -> k_constraint (MJB_FORK=1) or the serial chain (default)
-  for split, graph, fork in (("1", "0", "0"), ("1", "0", "1"), ("2", "0", "1"), ("3", "0", "1"), ("2", "1", "1"), ("3", "1", "1"), ("2", "1", "0")):
-    out = tmp_path / f"s{split}g{graph}f{fork}.npz"
-    env = dict(os.environ, MJB_SPLIT=split, MJB_FORK=fork)
+  for split, graph in (("1", "0"), ("2", "0"), ("3", "0"), ("2", "1"), ("3", "1")):
+    out = tmp_path / f"s{split}g{graph}.npz"
+    env = dict(os.environ, MJB_SPLIT=split)
     subprocess.check_call([sys.executable, str(script), root, scene, str(nworld), graph, str(out)], env=env)
-    outs[(split, graph, fork)] = np.load(out)
-  ref = outs[("1", "0", "0")]
+    outs[(split, graph)] = np.load(out)
+  ref = outs[("1", "0")]
   assert ref["nefc"].max() > 0 and ref["ncon"].max() > 0
   for key, got in outs.items():
     for f in ref.files:
-      np.testing.assert_array_equal(got[f], ref[f], err_msg=f"MJB_SPLIT={key[0]} graph={key[1]} MJB_FORK={key[2]}: {f}")
+      np.testing.assert_array_equal(got[f], ref[f], err_msg=f"MJB_SPLIT={key[0]} graph={key[1]}: {f}")
   # and the unsplit run agrees with the oracle (fp32 build) on the integer outputs after the same 6 steps from the same state
   import mujoco_warp_b200 as mjw
 

@@ -1,5 +1,5 @@
 """Per-kernel and whole-step timing of the humanoid benchmark state (deterministic: `warm` steps from the squat keyframe).
-usage: python tools/ktime.py [nworld] [warm] [reps]   (kernel variants are chosen by the MJB_* environment variables)"""
+usage: python tools/ktime.py [nworld] [warm] [reps]   (MJB_LIB selects the library build to time, KT_MODEL / KT_NCONMAX / KT_NJMAX the scene)"""
 import json
 import os
 import sys

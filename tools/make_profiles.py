@@ -107,8 +107,8 @@ def solver_lines():
   marks = [("set-up: layout, reductions, row evaluation helpers", 1)]
   for name, needle in (("mul_m", "// res = M vec"), ("update_constraint (force / state per row, J^T force)", "// force/state per row"), ("update_grad", "// grad = Ma"),
                        ("Hessian update in registers (newton_direction_reg)", "// Newton direction for nv <= 32"), ("update_search (dispatch, nv > 32 path)", "// H += sum_list"),
-                       ("line search", "template <bool ELL, int NW>\n__device__ __forceinline__ P3 eval_total"), ("CG direction", "// Conjugate-gradient direction"),
-                       ("kernel: staging, init_context, main loop, results", "template <bool ELL, bool BIG, bool CG, int NW>\n__global__")):
+                       ("line search", "template <bool ELL>\n__device__ __forceinline__ P3 eval_total"), ("CG direction", "// Conjugate-gradient direction"),
+                       ("kernel: staging, init_context, main loop, results", "template <bool ELL, bool BIG, bool CG, bool PLAIN = false, int NREG = 0>\n__global__")):
     pos = "\n".join(text).find(needle)
     if pos >= 0:
       marks.append((name, "\n".join(text)[:pos].count("\n") + 1))
