@@ -108,8 +108,10 @@ int mjb_implicit(const mjbModel* m, mjbData* d, void* stream);
 /* ctrl <- OU noise around ctrl_center (device array of nu floats, or NULL), reference cli.py:103-145 */
 int mjb_ctrl_noise(const mjbModel* m, mjbData* d, const float* ctrl_center, int step, float noise_std, float noise_rate, void* stream);
 
-/* profiling aid: runs ONE step with a CUDA-event pair around each of the 6 kernels (position, collision, constraint,
- * velocity, solver, integrate), synchronises, and writes the 6 durations in ms to ms_out (host pointer). */
+/* profiling aid: runs ONE step's kernel chain over all worlds on `stream` (not split over world halves), synchronises, and writes
+ * the durations in ms of its 6 stage groups to ms_out (host pointer, 6 floats): position, collision, constraint (with the CSR
+ * view of sparse models), velocity, solver (with the sensors), integrate (every integrator kernel).  The contact-counter resets
+ * run before the first event, so the durations cover kernels only.  RK4 models profile one forward pass and the Euler update. */
 int mjb_step_profile(const mjbModel* m, mjbData* d, void* stream, float* ms_out);
 
 /* worlds per SM that are resident at once (cudaOccupancyMaxActiveBlocksPerMultiprocessor times worlds per block) in the launch
@@ -117,7 +119,8 @@ int mjb_step_profile(const mjbModel* m, mjbData* d, void* stream, float* ms_out)
  * ceil(nworld / (SMs x worlds per SM)) rounds of one world's dependent chain. */
 int mjb_team_residency(const mjbModel* m, const mjbData* d, int* position_worlds, int* velocity_worlds);
 
-/* number of kernels the last mjb_* pipeline call launched (for bench.py's gpu_launches) */
+/* number of kernels launched by the calling thread's last mjb_* call that enqueues work, counted at each launch (memsets are not
+ * kernels and are not counted); bench.py's gpu_launches */
 int mjb_last_launch_count(void);
 const char* mjb_last_error(void);
 const char* mjb_version(void);

@@ -266,7 +266,9 @@ KERNEL_NAMES = ("position", "collision", "constraint", "velocity", "solver", "in
 
 
 def step_profile(m: Model, d: Data):
-  """One step with per-kernel CUDA-event timing; returns {kernel: ms}. Synchronises (profiling aid)."""
+  """One step's kernel chain over all worlds with a CUDA event after each stage group; returns {group: ms} for the groups of
+  KERNEL_NAMES.  `constraint` includes the CSR view of sparse models, `solver` the sensors, `integrate` every integrator kernel.
+  RK4 models profile one forward pass and the Euler update.  Synchronises (profiling aid)."""
   import ctypes
 
   out = (ctypes.c_float * 6)()

@@ -7,6 +7,7 @@ using std::min;
 #include <string>
 
 #include "../../include/mjb200.h"
+#include "mjb_launch.cuh"
 #include "mjb_types.cuh"
 
 struct mjbModel {
@@ -16,7 +17,6 @@ struct mjbModel {
 struct mjbData {
   DataDev dev;
   bool finalized;
-  size_t smem[6];
   // step pipelining over two world halves on two internal streams (overlaps each kernel's partial last wave with the
   // other half's kernels; worlds never interact, so the halves are independent apart from the shared contact-pool counter)
   cudaStream_t aux[8];
@@ -27,7 +27,6 @@ struct mjbData {
 
 namespace {
 thread_local std::string g_err;
-thread_local int g_launches = 0;
 int fail(const std::string& s) { g_err = s; return -1; }
 int check(cudaError_t e, const char* what) {
   if (e == cudaSuccess) return 0;
@@ -146,13 +145,13 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
   if (check(cudaMalloc(&d->dev.imp_qacc, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nv > 0 ? m->dev.nv : 1)), "cudaMalloc(imp_qacc)")) return -1;
   if (m->dev.integrator == INT_RK4 && !d->rk &&
       check(cudaMalloc(&d->rk, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nq + 3 * m->dev.nv + 2 * m->dev.na + 1)), "cudaMalloc(rk)")) return -1;
-  d->smem[0] = smem_position(m->dev, d->dev); d->smem[1] = smem_collision(m->dev, d->dev); d->smem[2] = smem_constraint(m->dev, d->dev);
-  d->smem[3] = smem_velocity(m->dev, d->dev); d->smem[4] = smem_solver(m->dev, d->dev); d->smem[5] = smem_integrate(m->dev);
+  const size_t smem[6] = {smem_position(m->dev, d->dev), smem_collision(m->dev, d->dev), smem_constraint(m->dev, d->dev),
+                          smem_velocity(m->dev, d->dev), smem_solver(m->dev, d->dev),    smem_integrate(m->dev)};
   static const char* names[6] = {"position", "collision", "constraint", "velocity", "solver", "integrate"};
   for (int i = 0; i < 6; i++)
-    if (d->smem[i] > kMaxSmem) {
+    if (smem[i] > kMaxSmem) {
       char buf[160];
-      snprintf(buf, sizeof buf, "%s kernel needs %zu B of shared memory per block (> %zu): model/njmax too large for this version", names[i], d->smem[i], kMaxSmem);
+      snprintf(buf, sizeof buf, "%s kernel needs %zu B of shared memory per block (> %zu): model/njmax too large for this version", names[i], smem[i], kMaxSmem);
       return fail(buf);
     }
   {
@@ -176,82 +175,96 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
   if (!m || !d || !m->finalized || !d->finalized) return fail("model/data not finalized"); \
   cudaStream_t s = (cudaStream_t)stream;                                             \
   g_launches = 0;
-#define MJB_LAUNCH(call, n) do { if (check((call), #call)) return -1; g_launches += (n); } while (0)
+#define MJB_LAUNCH(call) do { if (check((call), #call)) return -1; } while (0)
 
-int mjb_kinematics(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_KINEMATICS, s), 1); return 0; }
-int mjb_com_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_COM_POS, s), 1); return 0; }
-int mjb_camlight(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_CAMLIGHT, s), 1); return 0; }
-int mjb_crb(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_CRB, s), 1); return 0; }
-int mjb_transmission(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_TRANSMISSION, s), 1); return 0; }
-int mjb_collision(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(reset_contact_counters(d->dev, s), 0); MJB_LAUNCH(launch_collision(m->dev, d->dev, s), 1); return 0; }
+int mjb_kinematics(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_KINEMATICS, s)); return 0; }
+int mjb_com_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_COM_POS, s)); return 0; }
+int mjb_camlight(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_CAMLIGHT, s)); return 0; }
+int mjb_crb(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_CRB, s)); return 0; }
+int mjb_transmission(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_TRANSMISSION, s)); return 0; }
+int mjb_collision(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(reset_contact_counters(d->dev, s)); MJB_LAUNCH(launch_collision(m->dev, d->dev, s)); return 0; }
 int mjb_make_constraint(const mjbModel* m, mjbData* d, void* stream) {
   MJB_ENTER();
-  MJB_LAUNCH(launch_constraint(m->dev, d->dev, s), 1);
-  if (d->dev.njmax_nnz > 0) MJB_LAUNCH(launch_efc_csr(m->dev, d->dev, s), 1);
+  MJB_LAUNCH(launch_constraint(m->dev, d->dev, s));
+  if (d->dev.njmax_nnz > 0) MJB_LAUNCH(launch_efc_csr(m->dev, d->dev, s));
   return 0;
 }
-int mjb_fwd_velocity(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_VELOCITY, s), 1); return 0; }
-int mjb_fwd_actuation(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_ACTUATION, s), 1); return 0; }
-int mjb_fwd_acceleration(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_ACCELERATION, s), 1); return 0; }
-int mjb_factor_m(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_FACTOR_ONLY, s), 1); return 0; }
-int mjb_com_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_COMVEL, s), 1); return 0; }
-int mjb_passive(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_PASSIVE, s), 1); return 0; }
-int mjb_rne(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_RNE, s), 1); return 0; }
+int mjb_fwd_velocity(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_VELOCITY, s)); return 0; }
+int mjb_fwd_actuation(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_ACTUATION, s)); return 0; }
+int mjb_fwd_acceleration(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_ACCELERATION, s)); return 0; }
+int mjb_factor_m(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_FACTOR_ONLY, s)); return 0; }
+int mjb_com_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_COMVEL, s)); return 0; }
+int mjb_passive(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_PASSIVE, s)); return 0; }
+int mjb_rne(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_RNE, s)); return 0; }
 int mjb_solve_m(const mjbModel* m, mjbData* d, float* x, const float* y, void* stream) {
   MJB_ENTER();
   if (!x || !y) return fail("mjb_solve_m: null vector");
-  MJB_LAUNCH(launch_solve_m(m->dev, d->dev, x, y, s), 1);
+  MJB_LAUNCH(launch_solve_m(m->dev, d->dev, x, y, s));
   return 0;
 }
 int mjb_mul_m(const mjbModel* m, mjbData* d, float* res, const float* vec, void* stream) {
   MJB_ENTER();
   if (!res || !vec) return fail("mjb_mul_m: null vector");
-  MJB_LAUNCH(launch_mul_m(m->dev, d->dev, res, vec, s), 1);
+  MJB_LAUNCH(launch_mul_m(m->dev, d->dev, res, vec, s));
   return 0;
 }
 int mjb_contact_force(const mjbModel* m, mjbData* d, const int* contact_ids, int n, int to_world_frame, float* force, void* stream) {
   MJB_ENTER();
   if (n > 0 && (!contact_ids || !force)) return fail("mjb_contact_force: null array");
-  MJB_LAUNCH(launch_contact_force(m->dev, d->dev, contact_ids, n, to_world_frame, force, s), 1);
+  MJB_LAUNCH(launch_contact_force(m->dev, d->dev, contact_ids, n, to_world_frame, force, s));
   return 0;
 }
-int mjb_sensor_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 1, s), 1); return 0; }
-int mjb_sensor_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 2, s), 1); return 0; }
-int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 4, s), 1); return 0; }
-int mjb_solve(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_solver(m->dev, d->dev, s), 1); return 0; }
-int mjb_euler(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_integrate(m->dev, d->dev, INT_EULER, s), 1); return 0; }
-int mjb_implicit(const mjbModel* m, mjbData* d, void* stream) {
-  MJB_ENTER();
-  if (m->dev.integrator != INT_IMPLICIT && m->dev.integrator != INT_IMPLICITFAST) return fail("mjb_implicit: the model's integrator is Euler / RK4 (the factor-and-solve scratch is sized by the integrator the model was created with)");
-  if (m->dev.integrator == INT_IMPLICIT && smem_implicit(m->dev) > kMaxSmem) return fail("implicit integrator: the velocity-derivative scratch (18 x nbody x 32 floats) exceeds one block's shared memory");
-  MJB_LAUNCH(launch_integrate(m->dev, d->dev, m->dev.integrator == INT_IMPLICIT ? INT_IMPLICIT : INT_IMPLICITFAST, s), m->dev.integrator == INT_IMPLICIT ? 2 : 1);
-  return 0;
-}
+int mjb_sensor_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 1, s)); return 0; }
+int mjb_sensor_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 2, s)); return 0; }
+int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 4, s)); return 0; }
+int mjb_solve(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_solver(m->dev, d->dev, s)); return 0; }
+int mjb_euler(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_integrate(m->dev, d->dev, INT_EULER, s)); return 0; }
 
 // which stages a pipeline call runs
 enum { RUN_POSITION = 1, RUN_VELOCITY = 2, RUN_SOLVER = 4, RUN_EULER = 8 };
 
-static int chain(const mjbModel* m, const DataDev& dd, int what, cudaStream_t s) {
+// The kernels of the stages in `what` for dd's world range.  With `marks` (six events), the end of each stage group is recorded
+// in the order of forward.KERNEL_NAMES: position, collision, constraint (with the CSR view), velocity, solver (with the sensors),
+// integrate (every integrator kernel).
+static int chain(const mjbModel* m, const DataDev& dd, int what, cudaStream_t s, cudaEvent_t* marks = nullptr) {
+#define MJB_MARK(i) do { if (marks && check(cudaEventRecord(marks[i], s), "cudaEventRecord")) return -1; } while (0)
   if (what & RUN_POSITION) {
     // forward.py:635-677 with factorize=False: kinematics, com_pos, camlight, crb, collision, make_constraint, transmission
-    MJB_LAUNCH(launch_position(m->dev, dd, STG_KINEMATICS | STG_COM_POS | STG_CAMLIGHT | STG_CRB | STG_TRANSMISSION, s), 1);
-    MJB_LAUNCH(launch_collision(m->dev, dd, s), 1);
-    MJB_LAUNCH(launch_constraint(m->dev, dd, s), 1);
-    if (dd.njmax_nnz > 0) MJB_LAUNCH(launch_efc_csr(m->dev, dd, s), 1);  // sparse models: the reference's CSR arrays next to the dense rows
+    MJB_LAUNCH(launch_position(m->dev, dd, STG_KINEMATICS | STG_COM_POS | STG_CAMLIGHT | STG_CRB | STG_TRANSMISSION, s));
+    MJB_MARK(0);
+    MJB_LAUNCH(launch_collision(m->dev, dd, s));
+    MJB_MARK(1);
+    MJB_LAUNCH(launch_constraint(m->dev, dd, s));
+    if (dd.njmax_nnz > 0) MJB_LAUNCH(launch_efc_csr(m->dev, dd, s));  // sparse models: the reference's CSR arrays next to the dense rows
+    MJB_MARK(2);
   }
-  if (what & RUN_VELOCITY) MJB_LAUNCH(launch_velocity(m->dev, dd, STG_VELOCITY | STG_ACTUATION | STG_ACCELERATION, s), 1);
-  if (what & RUN_SOLVER) MJB_LAUNCH(launch_solver(m->dev, dd, s), 1);
-  // sensors of all three stages in one launch after the solver (forward.py:1350-1365 interleaves them; their inputs are final by now)
-  if ((what & RUN_SOLVER) && m->dev.nsensor > 0) MJB_LAUNCH(launch_sensor(m->dev, dd, 7, s), 1);
+  if (what & RUN_VELOCITY) {
+    MJB_LAUNCH(launch_velocity(m->dev, dd, STG_VELOCITY | STG_ACTUATION | STG_ACCELERATION, s));
+    MJB_MARK(3);
+  }
+  if (what & RUN_SOLVER) {
+    MJB_LAUNCH(launch_solver(m->dev, dd, s));
+    // sensors of all three stages in one launch after the solver (forward.py:1350-1365 interleaves them; their inputs are final by now)
+    if (m->dev.nsensor > 0) MJB_LAUNCH(launch_sensor(m->dev, dd, 7, s));
+    MJB_MARK(4);
+  }
   if (what & RUN_EULER) {
     if (m->dev.integrator == INT_IMPLICIT && smem_implicit(m->dev) > kMaxSmem) return fail("implicit integrator: the velocity-derivative scratch (18 x nbody x 32 floats) exceeds one block's shared memory");
-    MJB_LAUNCH(launch_integrate(m->dev, dd, -1, s), m->dev.integrator == INT_IMPLICIT ? 2 : 1);
+    MJB_LAUNCH(launch_integrate(m->dev, dd, -1, s));
+    MJB_MARK(5);
   }
+#undef MJB_MARK
   return 0;
 }
 
+int mjb_implicit(const mjbModel* m, mjbData* d, void* stream) {
+  MJB_ENTER();
+  if (m->dev.integrator != INT_IMPLICIT && m->dev.integrator != INT_IMPLICITFAST) return fail("mjb_implicit: the model's integrator is Euler / RK4 (the factor-and-solve scratch is sized by the integrator the model was created with)");
+  return chain(m, d->dev, RUN_EULER, s);
+}
+
 static int pipeline(const mjbModel* m, mjbData* d, int what, cudaStream_t s) {
-  if (what & RUN_POSITION) MJB_LAUNCH(reset_contact_counters(d->dev, s), 0);
+  if (what & RUN_POSITION) MJB_LAUNCH(reset_contact_counters(d->dev, s));
   if (d->nsplit < 2) return chain(m, d->dev, what, s);
   // fork: both halves wait for everything queued on the caller's stream, run their own kernel chain, and are joined back
   if (check(cudaEventRecord(d->ev_fork, s), "cudaEventRecord")) return -1;
@@ -275,7 +288,7 @@ static int rk4_after_forward(const mjbModel* m, mjbData* d, cudaStream_t s) {
   if (!d->rk) return fail("Runge-Kutta scratch missing: data was finalized against a model whose integrator is not RK4");
   for (int stage = 0; stage < 4; stage++) {
     if (stage > 0 && pipeline(m, d, RUN_POSITION | RUN_VELOCITY | RUN_SOLVER, s)) return -1;
-    MJB_LAUNCH(launch_rk_stage(m->dev, d->dev, d->rk, stage, s), 1);
+    MJB_LAUNCH(launch_rk_stage(m->dev, d->dev, d->rk, stage, s));
   }
   return 0;
 }
@@ -289,28 +302,18 @@ int mjb_step(const mjbModel* m, mjbData* d, void* stream) {
   return pipeline(m, d, RUN_POSITION | RUN_VELOCITY | RUN_SOLVER | RUN_EULER, s);
 }
 int mjb_step_profile(const mjbModel* m, mjbData* d, void* stream, float* ms_out) {
-  // one step with a CUDA event pair around every kernel; synchronises (profiling aid, not the hot path)
   MJB_ENTER();
+  // the step's kernel chain over all worlds on the caller's stream, between event ev[0] and the six stage-group events
   cudaEvent_t ev[7];
-  for (int i = 0; i < 7; i++) if (check(cudaEventCreate(&ev[i]), "cudaEventCreate")) return -1;
-  cudaEventRecord(ev[0], s);
-  MJB_LAUNCH(launch_position(m->dev, d->dev, STG_KINEMATICS | STG_COM_POS | STG_CAMLIGHT | STG_CRB | STG_TRANSMISSION, s), 1);
-  cudaEventRecord(ev[1], s);
-  MJB_LAUNCH(reset_contact_counters(d->dev, s), 0);
-  MJB_LAUNCH(launch_collision(m->dev, d->dev, s), 1);
-  cudaEventRecord(ev[2], s);
-  MJB_LAUNCH(launch_constraint(m->dev, d->dev, s), 1);
-  cudaEventRecord(ev[3], s);
-  MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_VELOCITY | STG_ACTUATION | STG_ACCELERATION, s), 1);
-  cudaEventRecord(ev[4], s);
-  MJB_LAUNCH(launch_solver(m->dev, d->dev, s), 1);
-  cudaEventRecord(ev[5], s);
-  MJB_LAUNCH(launch_integrate(m->dev, d->dev, -1, s), 1);
-  cudaEventRecord(ev[6], s);
-  if (check(cudaEventSynchronize(ev[6]), "cudaEventSynchronize")) return -1;
-  for (int i = 0; i < 6; i++) cudaEventElapsedTime(&ms_out[i], ev[i], ev[i + 1]);
-  for (int i = 0; i < 7; i++) cudaEventDestroy(ev[i]);
-  return 0;
+  int n = 0, rc = 0;
+  while (n < 7 && !(rc = check(cudaEventCreate(&ev[n]), "cudaEventCreate"))) n++;
+  if (!rc) rc = check(reset_contact_counters(d->dev, s), "reset_contact_counters");
+  if (!rc) rc = check(cudaEventRecord(ev[0], s), "cudaEventRecord");
+  if (!rc) rc = chain(m, d->dev, RUN_POSITION | RUN_VELOCITY | RUN_SOLVER | RUN_EULER, s, ev + 1);
+  if (!rc) rc = check(cudaEventSynchronize(ev[6]), "cudaEventSynchronize");
+  for (int i = 0; i < 6 && !rc; i++) rc = check(cudaEventElapsedTime(&ms_out[i], ev[i], ev[i + 1]), "cudaEventElapsedTime");
+  for (int i = 0; i < n; i++) cudaEventDestroy(ev[i]);
+  return rc;
 }
 int mjb_team_residency(const mjbModel* m, const mjbData* d, int* position_worlds, int* velocity_worlds) {
   if (!m || !d || !m->finalized || !d->finalized) return fail("model/data not finalized");
@@ -321,7 +324,7 @@ int mjb_team_residency(const mjbModel* m, const mjbData* d, int* position_worlds
 }
 int mjb_ctrl_noise(const mjbModel* m, mjbData* d, const float* ctrl_center, int step, float noise_std, float noise_rate, void* stream) {
   MJB_ENTER();
-  MJB_LAUNCH(launch_ctrl_noise(m->dev, d->dev, ctrl_center, step, noise_std, noise_rate, s), 1);
+  MJB_LAUNCH(launch_ctrl_noise(m->dev, d->dev, ctrl_center, step, noise_std, noise_rate, s));
   return 0;
 }
 

@@ -16,6 +16,7 @@
 #include "mjb_ccd.cuh"
 #include "mjb_colliders.cuh"
 
+#include "mjb_launch.cuh"
 #include "mjb_math.cuh"
 #include "mjb_team.cuh"
 #include "mjb_types.cuh"
@@ -520,22 +521,11 @@ cudaError_t LAUNCH_NAME(const ModelDev& m, const DataDev& d, cudaStream_t s) {
 #ifndef MJB_COLLISION_MESH_TU
   if (m.nmesh > 0) return launch_collision_mesh(m, d, s);  // models with mesh geoms run the CCD_MESH build of this kernel
 #endif
-  const size_t smem = SMEM_NAME(m, d);
-  static size_t configured4[4] = {0, 0, 0, 0};
 #ifdef MJB_COLLISION_MESH_TU
-  const int full = 1;
   void (*kern)(ModelDev, DataDev) = m.batched ? k_collision<8, true> : k_collision<8, false>;
 #else
-  const int full = m.has_multicontact_geom ? 1 : 0;
-  void (*kern)(ModelDev, DataDev) = full ? (m.batched ? k_collision<8, true> : k_collision<8, false>) : (m.batched ? k_collision<2, true> : k_collision<2, false>);
+  void (*kern)(ModelDev, DataDev) = m.has_multicontact_geom ? (m.batched ? k_collision<8, true> : k_collision<8, false>) : (m.batched ? k_collision<2, true> : k_collision<2, false>);
 #endif
-  const int ci = full + 2 * (m.batched ? 1 : 0);
-  if (smem > 48 * 1024 && smem > configured4[ci]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    configured4[ci] = smem;
-  }
   const int grid = (d.wn + collision_wpb() - 1) / collision_wpb();
-  kern<<<grid, collision_wpb() * 32, smem, s>>>(m, d);
-  return cudaGetLastError();
+  return launch(kern, grid, collision_wpb() * 32, SMEM_NAME(m, d), s, m, d);
 }

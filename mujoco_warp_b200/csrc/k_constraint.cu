@@ -12,6 +12,7 @@
 // single coalesced store, J*qvel is a warp-shuffle reduction; the per-row impedance / reference math of the contact rows runs
 // afterwards with lanes = rows of the 32-contact batch (phase C), so its eight per-row stores are coalesced over consecutive rows.
 
+#include "mjb_launch.cuh"
 #include "mjb_math.cuh"
 #include "mjb_types.cuh"
 
@@ -548,17 +549,8 @@ constexpr int constraint_wpb() { return 2; }
 size_t smem_constraint(const ModelDev& m, const DataDev& d) { return (size_t)con_layout(m, d).total * sizeof(float) * constraint_wpb(); }
 
 cudaError_t launch_constraint(const ModelDev& m, const DataDev& d, cudaStream_t s) {
-  const size_t smem = smem_constraint(m, d);
-  static size_t configured[4] = {0, 0, 0, 0};
-  const int eq = (m.neq > 0 || m.nlimit_ball > 0 || m.ntendon > 0) ? 1 : 0;
+  const bool eq = m.neq > 0 || m.nlimit_ball > 0 || m.ntendon > 0;
   void (*kern)(ModelDev, DataDev) = eq ? (m.batched ? k_constraint<true, true> : k_constraint<true, false>) : (m.batched ? k_constraint<false, true> : k_constraint<false, false>);
-  const int ci = eq + 2 * (m.batched ? 1 : 0);
-  if (smem > 48 * 1024 && smem > configured[ci]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    configured[ci] = smem;
-  }
   const int grid = (d.wn + constraint_wpb() - 1) / constraint_wpb();
-  kern<<<grid, constraint_wpb() * 32, smem, s>>>(m, d);
-  return cudaGetLastError();
+  return launch(kern, grid, constraint_wpb() * 32, smem_constraint(m, d), s, m, d);
 }

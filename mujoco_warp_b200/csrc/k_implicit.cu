@@ -13,6 +13,7 @@
 // the last dof to the first like the reference's (U unit upper, L lower): entries outside the D-structure never fill in, because two dofs
 // that are both ancestors of a third lie on one chain -- so the dense elimination reproduces the sparse one.  Results: Data.qLU (the factors,
 // D-structure) and the solved acceleration for the advance kernel (k_integrate.cu).
+#include "mjb_launch.cuh"
 #include "mjb_math.cuh"
 #include "mjb_types.cuh"
 
@@ -259,15 +260,5 @@ k_implicit(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
 size_t smem_implicit(const ModelDev& m) { return (size_t)imp_layout(m).total * sizeof(float); }
 
 cudaError_t launch_implicit_solve(const ModelDev& m, const DataDev& d, float* qacc_out, cudaStream_t s) {
-  const size_t smem = smem_implicit(m);
-  static size_t configured[2] = {0, 0};
-  auto kern = m.batched ? k_implicit<true> : k_implicit<false>;
-  const int ci = m.batched ? 1 : 0;
-  if (smem > 48 * 1024 && smem > configured[ci]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    configured[ci] = smem;
-  }
-  kern<<<d.wn, 32, smem, s>>>(m, d, qacc_out);
-  return cudaGetLastError();
+  return launch(m.batched ? k_implicit<true> : k_implicit<false>, d.wn, 32, smem_implicit(m), s, m, d, qacc_out);
 }

@@ -6,6 +6,7 @@
 // derivative.py:38-176 _qderiv_actuator_passive_vel, :178-245 moment^T vel moment scatter, :221-245 damping) factors
 // M - dt*qDeriv instead.  cli.py:103-145 _ctrl_noise.
 #include "mjb_chol.cuh"
+#include "mjb_launch.cuh"
 #include "mjb_math.cuh"
 #include "mjb_types.cuh"
 
@@ -20,7 +21,7 @@ __host__ __device__ inline int int_words(const ModelDev& m) {
 }
 
 template <bool BAT>
-__global__ void __launch_bounds__(MJB_WARPS_PER_BLOCK * 32)
+__global__ void __launch_bounds__(32)
 k_euler(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d, int integrator) {
   extern __shared__ float smem[];
   const int lane = threadIdx.x, warp = 0;  // one warp per block: the world index is block-uniform
@@ -313,51 +314,31 @@ k_rk_stage(const __grid_constant__ ModelDev m, const __grid_constant__ DataDev d
 
 }  // namespace
 
-size_t smem_integrate(const ModelDev& m) { return (size_t)int_words(m) * sizeof(float) * MJB_WARPS_PER_BLOCK; }
+size_t smem_integrate(const ModelDev& m) { return (size_t)int_words(m) * sizeof(float); }
 
 // integrator: INT_EULER / INT_IMPLICITFAST / INT_IMPLICIT, or -1 for the model's own (RK4 models advance with Euler here, forward.py:1411)
 cudaError_t launch_integrate(const ModelDev& m, const DataDev& d, int integrator, cudaStream_t s) {
   if (integrator < 0) integrator = (m.integrator == INT_IMPLICITFAST || m.integrator == INT_IMPLICIT) ? m.integrator : INT_EULER;
   const bool solve = integrator == INT_IMPLICITFAST || integrator == INT_IMPLICIT || !(m.disableflags & (DSBL_EULERDAMP | DSBL_DAMPER));
-  if (integrator == INT_IMPLICIT) {
-    cudaError_t e = launch_implicit_solve(m, d, d.imp_qacc, s);
-    if (e != cudaSuccess) return e;
-  }
-  auto next_activation = [&]() -> cudaError_t {  // after the integrator kernel: it reads the activations of the step
-    if (m.na <= 0 || m.nu <= 0) return cudaGetLastError();
-    const long n = (long)d.wn * m.nu;
-    if (m.batched) k_next_act<true><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(m, d);
-    else k_next_act<false><<<(unsigned)((n + 255) / 256), 256, 0, s>>>(m, d);
-    return cudaGetLastError();
-  };
+  cudaError_t e = integrator == INT_IMPLICIT ? launch_implicit_solve(m, d, d.imp_qacc, s) : cudaSuccess;
+  if (e != cudaSuccess) return e;
   if (!solve && m.njnt > 0) {
     const long n = (long)d.wn * m.njnt;
-    k_euler_flat<<<(unsigned)((n + 255) / 256), 256, 0, s>>>(m, d);
-    return next_activation();
+    e = launch(k_euler_flat, (unsigned)((n + 255) / 256), 256, 0, s, m, d);
+  } else {
+    e = launch(m.batched ? k_euler<true> : k_euler<false>, d.wn, 32, smem_integrate(m), s, m, d, integrator);
   }
-  const size_t smem = smem_integrate(m);
-  static size_t configured2[2] = {0, 0};
-  size_t& configured = configured2[m.batched ? 1 : 0];
-  if (smem > 48 * 1024 && smem > configured) {
-    cudaError_t e = cudaFuncSetAttribute(m.batched ? k_euler<true> : k_euler<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    configured = smem;
-  }
-  const int grid = d.wn;
-  if (m.batched) k_euler<true><<<grid, MJB_WARPS_PER_BLOCK * 32, smem, s>>>(m, d, integrator);
-  else k_euler<false><<<grid, MJB_WARPS_PER_BLOCK * 32, smem, s>>>(m, d, integrator);
-  return next_activation();
+  if (e != cudaSuccess || m.na <= 0 || m.nu <= 0) return e;
+  const long n = (long)d.wn * m.nu;  // after the integrator kernel: it reads the activations of the step
+  return launch(m.batched ? k_next_act<true> : k_next_act<false>, (unsigned)((n + 255) / 256), 256, 0, s, m, d);
 }
 
 cudaError_t launch_ctrl_noise(const ModelDev& m, const DataDev& d, const float* ctrl_center, int step, float std, float rate, cudaStream_t s) {
   const int n = d.nworld * m.nu;
   if (n == 0) return cudaSuccess;
-  if (m.batched) k_ctrl_noise<true><<<(n + 255) / 256, 256, 0, s>>>(m, d, ctrl_center, step, std, rate);
-  else k_ctrl_noise<false><<<(n + 255) / 256, 256, 0, s>>>(m, d, ctrl_center, step, std, rate);
-  return cudaGetLastError();
+  return launch(m.batched ? k_ctrl_noise<true> : k_ctrl_noise<false>, (n + 255) / 256, 256, 0, s, m, d, ctrl_center, step, std, rate);
 }
 
 cudaError_t launch_rk_stage(const ModelDev& m, const DataDev& d, float* rk, int stage, cudaStream_t s) {
-  k_rk_stage<<<d.nworld, 32, 0, s>>>(m, d, rk, stage);
-  return cudaGetLastError();
+  return launch(k_rk_stage, d.nworld, 32, 0, s, m, d, rk, stage);
 }

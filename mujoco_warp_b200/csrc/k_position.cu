@@ -398,41 +398,10 @@ k_position(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
 
 }  // namespace
 
-static void (*pos_kernel(const ModelDev& m, int lpw))(ModelDev, DataDev, int) {
+static TeamKernel pos_kernel(const ModelDev& m, int lpw) {
   return m.batched ? k_position<32, true> : lpw == 8 ? k_position<8, false> : lpw == 16 ? k_position<16, false> : k_position<32, false>;
 }
 
-static TeamShape pos_shape(const ModelDev& m, const DataDev& d) {
-  TeamShape t = team_shape((size_t)pos_layout(m).total, d.wn, [&](int lpw) { return kernel_regs(pos_kernel(m, lpw)); });
-  if (m.batched && t.lpw != 32) { t = team_shape_fixed((size_t)pos_layout(m).total, 32, 2); }
-  return t;
-}
-size_t smem_position(const ModelDev& m, const DataDev& d) { return pos_shape(m, d).block_bytes; }
-
-// the kernel instance for the launch shape, configured on its first use
-static cudaError_t pos_configured(const ModelDev& m, const TeamShape& t, void (**kern)(ModelDev, DataDev, int)) {
-  static TeamConfig configured[4];
-  const int lpw = t.lpw, ki = m.batched ? 3 : lpw == 8 ? 0 : lpw == 16 ? 1 : 2;
-  *kern = pos_kernel(m, lpw);
-  return team_configure(*kern, t.block_bytes, &configured[ki]);
-}
-
-cudaError_t launch_position(const ModelDev& m, const DataDev& d, int mask, cudaStream_t s) {
-  const TeamShape t = pos_shape(m, d);
-  void (*kern)(ModelDev, DataDev, int);
-  cudaError_t e = pos_configured(m, t, &kern);
-  if (e != cudaSuccess) return e;
-  const int G = 32 / t.lpw, ngroups = (d.wn + G - 1) / G, grid = (ngroups + t.wpb - 1) / t.wpb;
-  kern<<<grid, 32 * t.wpb, t.block_bytes, s>>>(m, d, mask);
-  return cudaGetLastError();
-}
-
-cudaError_t resident_worlds_position(const ModelDev& m, const DataDev& d, int* worlds) {
-  const TeamShape t = pos_shape(m, d);
-  void (*kern)(ModelDev, DataDev, int);
-  int blocks = 0;
-  cudaError_t e = pos_configured(m, t, &kern);
-  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, 32 * t.wpb, t.block_bytes);
-  *worlds = blocks * t.wpb * (32 / t.lpw);
-  return e;
-}
+size_t smem_position(const ModelDev& m, const DataDev& d) { return team_shape(m, d.wn, pos_layout(m).total, pos_kernel).block_bytes; }
+cudaError_t launch_position(const ModelDev& m, const DataDev& d, int mask, cudaStream_t s) { return team_launch(m, d, pos_layout(m).total, pos_kernel, mask, s); }
+cudaError_t resident_worlds_position(const ModelDev& m, const DataDev& d, int* worlds) { return team_resident_worlds(m, d, pos_layout(m).total, pos_kernel, worlds); }

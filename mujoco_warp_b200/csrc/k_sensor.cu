@@ -6,6 +6,7 @@
 // smooth.py:1743 rne_postconstraint (cfrc_ext from applied wrenches, body-to-body connect / weld equalities and contacts; cacc including
 // qacc; cfrc_int accumulated up the tree).  Every input a position- or velocity-stage sensor reads is final once its stage has run, so one launch after
 // the solver evaluates all three stages (the stage mask lets sensor_pos / sensor_vel / sensor_acc be called on their own).
+#include "mjb_launch.cuh"
 #include "mjb_math.cuh"
 #include "mjb_types.cuh"
 
@@ -437,7 +438,5 @@ k_sensor(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d,
 
 cudaError_t launch_sensor(const ModelDev& m, const DataDev& d, int stages, cudaStream_t s) {
   if (m.nsensor == 0) return cudaSuccess;
-  if (m.batched) k_sensor<true><<<d.wn, 32, (size_t)12 * m.nbody * sizeof(float), s>>>(m, d, stages);
-  else k_sensor<false><<<d.wn, 32, (size_t)12 * m.nbody * sizeof(float), s>>>(m, d, stages);
-  return cudaGetLastError();
+  return launch(m.batched ? k_sensor<true> : k_sensor<false>, d.wn, 32, (size_t)12 * m.nbody * sizeof(float), s, m, d, stages);
 }

@@ -16,6 +16,7 @@
 // in the default instantiation; k_solver<true> adds elliptic cones (solver.py:286-477 zones, :957-1015 per-contact
 // quads, :2443-2565 cone Hessian) with the Hessian rebuilt from M every iteration like the reference's elliptic path.
 #include "mjb_chol.cuh"
+#include "mjb_launch.cuh"
 #include "mjb_linesearch.cuh"
 #include "mjb_team.cuh"
 #include "mjb_math.cuh"
@@ -718,30 +719,21 @@ size_t smem_solver(const ModelDev& m, const DataDev& d) { return (size_t)sol_lay
 // One warp per world.  The "big" instantiation (packed Hessian and factor worked on in shared memory, Jacobian rows read through L2,
 // CSR inertia) is the path above nv = 32.
 cudaError_t launch_solver(const ModelDev& m, const DataDev& d, cudaStream_t s) {
-  const size_t smem = smem_solver(m, d);
   const int ell = m.cone == CONE_ELLIPTIC ? 1 : 0, big = m.nv > 32 ? 1 : 0, cg = m.solver == SOL_CG ? 1 : 0;
   const int which = 4 * cg + 2 * big + ell;
-  static size_t configured[12] = {0};
   static void (*const kerns[8])(ModelDev, DataDev) = {
     k_solver<false, false, false>, k_solver<true, false, false>, k_solver<false, true, false>, k_solver<true, true, false>,
     k_solver<false, false, true>,  k_solver<true, false, true>,  k_solver<false, true, true>,  k_solver<true, true, true>};
   void (*kern)(ModelDev, DataDev) = kerns[which];
-  int ci = which;
   // no equality and no friction-loss rows possible: the instantiation with ne = nf = 0 compiled in (humanoid solver 202 -> 181 us: the
   // line-search loops lose two of their three row kinds, and with them instructions and instruction-cache footprint)
   const bool plain = m.neq == 0 && m.nfricdof == 0 && m.ntenfric == 0 && m.ntendon == 0;
   if (which == 0 && plain) {
-    kern = k_solver<false, false, false, true>; ci = 8;
+    kern = k_solver<false, false, false, true>;
     // ... and the register-row size fixed (one Hessian / Cholesky variant in the kernel instead of five: 182 -> 178 us)
-    if (m.nv > 24 && m.nv <= 28 && d.nv_pad == 28) { kern = k_solver<false, false, false, true, 28>; ci = 9; }
-    else if (m.nv > 28 && d.nv_pad == 32) { kern = k_solver<false, false, false, true, 32>; ci = 10; }
+    if (m.nv > 24 && m.nv <= 28 && d.nv_pad == 28) kern = k_solver<false, false, false, true, 28>;
+    else if (m.nv > 28 && d.nv_pad == 32) kern = k_solver<false, false, false, true, 32>;
   }
-  if (which == 2 && plain) { kern = k_solver<false, true, false, true>; ci = 11; }  // nv > 32 (unitree G1, three_humanoids)
-  if (smem > 48 * 1024 && smem > configured[ci]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e != cudaSuccess) return e;
-    configured[ci] = smem;
-  }
-  kern<<<d.wn, 32, smem, s>>>(m, d);
-  return cudaGetLastError();
+  if (which == 2 && plain) kern = k_solver<false, true, false, true>;  // nv > 32 (unitree G1, three_humanoids)
+  return launch(kern, d.wn, 32, smem_solver(m, d), s, m, d);
 }

@@ -3,6 +3,7 @@
 // Replaces (reference, /root/reference/mujoco_warp/_src/): smooth.py:3214 solve_m (x = M^-1 y through the per-tree factor kept
 // in Data.qLD; the reference launches one tile kernel per block size) and support.py:153-256 mul_m (res = M vec through the
 // symmetric gather tables of io.py:1029-1050).  One warp per world, like every other stage.
+#include "mjb_launch.cuh"
 #include "mjb_math.cuh"
 #include "mjb_types.cuh"
 
@@ -167,20 +168,16 @@ __global__ void k_contact_force(const __grid_constant__ ModelDev m, const __grid
 }  // namespace
 
 cudaError_t launch_solve_m(const ModelDev& m, const DataDev& d, float* x, const float* y, cudaStream_t s) {
-  k_solve_m<<<d.wn, 32, (m.nv + 4) * sizeof(float), s>>>(m, d, x, y);
-  return cudaGetLastError();
+  return launch(k_solve_m, d.wn, 32, (m.nv + 4) * sizeof(float), s, m, d, x, y);
 }
 cudaError_t launch_mul_m(const ModelDev& m, const DataDev& d, float* res, const float* vec, cudaStream_t s) {
-  k_mul_m<<<d.wn, 32, (m.nv + 4) * sizeof(float), s>>>(m, d, res, vec);
-  return cudaGetLastError();
+  return launch(k_mul_m, d.wn, 32, (m.nv + 4) * sizeof(float), s, m, d, res, vec);
 }
 cudaError_t launch_contact_force(const ModelDev& m, const DataDev& d, const int* contact_ids, int n, int to_world, float* out, cudaStream_t s) {
   if (n <= 0) return cudaSuccess;
-  k_contact_force<<<(n + 127) / 128, 128, 0, s>>>(m, d, contact_ids, n, to_world, out);
-  return cudaGetLastError();
+  return launch(k_contact_force, (n + 127) / 128, 128, 0, s, m, d, contact_ids, n, to_world, out);
 }
 
 cudaError_t launch_efc_csr(const ModelDev& m, const DataDev& d, cudaStream_t s) {
-  k_efc_csr<<<d.wn, 32, 0, s>>>(m, d);
-  return cudaGetLastError();
+  return launch(k_efc_csr, d.wn, 32, 0, s, m, d);
 }

@@ -490,47 +490,15 @@ k_velocity(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
 }  // namespace
 
 template <bool PEXT>
-static void (*vel_kernel(int lpw, bool bat))(ModelDev, DataDev, int) {
+static TeamKernel vel_kernel(int lpw, bool bat) {
   if (bat) return k_velocity<PEXT, 32, true>;
   return lpw == 8 ? k_velocity<PEXT, 8, false> : lpw == 16 ? k_velocity<PEXT, 16, false> : k_velocity<PEXT, 32, false>;
 }
 // has_gravcomp also flags free / ball joint springs (io.py put_model); tendons live in the same instantiation
-static bool vel_ext(const ModelDev& m) { return m.has_gravcomp || m.ntendon > 0; }
-static void (*vel_kernel(const ModelDev& m, int lpw))(ModelDev, DataDev, int) {
-  return vel_ext(m) ? vel_kernel<true>(lpw, m.batched) : vel_kernel<false>(lpw, m.batched);
+static TeamKernel vel_kernel(const ModelDev& m, int lpw) {
+  return m.has_gravcomp || m.ntendon > 0 ? vel_kernel<true>(lpw, m.batched) : vel_kernel<false>(lpw, m.batched);
 }
 
-static TeamShape vel_shape(const ModelDev& m, const DataDev& d) {
-  TeamShape t = team_shape((size_t)vel_layout(m).total, d.wn, [&](int lpw) { return kernel_regs(vel_kernel(m, lpw)); });
-  if (m.batched && t.lpw != 32) t = team_shape_fixed((size_t)vel_layout(m).total, 32, 2);
-  return t;
-}
-size_t smem_velocity(const ModelDev& m, const DataDev& d) { return vel_shape(m, d).block_bytes; }
-
-// the kernel instance for the launch shape, configured on its first use
-static cudaError_t vel_configured(const ModelDev& m, const TeamShape& t, void (**kern)(ModelDev, DataDev, int)) {
-  static TeamConfig configured[2][4];
-  const int ext = vel_ext(m) ? 1 : 0, ki = m.batched ? 3 : t.lpw == 8 ? 0 : t.lpw == 16 ? 1 : 2;
-  *kern = vel_kernel(m, t.lpw);
-  return team_configure(*kern, t.block_bytes, &configured[ext][ki]);
-}
-
-cudaError_t launch_velocity(const ModelDev& m, const DataDev& d, int mask, cudaStream_t s) {
-  const TeamShape t = vel_shape(m, d);
-  void (*kern)(ModelDev, DataDev, int);
-  cudaError_t e = vel_configured(m, t, &kern);
-  if (e != cudaSuccess) return e;
-  const int G = 32 / t.lpw, ngroups = (d.wn + G - 1) / G, grid = (ngroups + t.wpb - 1) / t.wpb;
-  kern<<<grid, 32 * t.wpb, t.block_bytes, s>>>(m, d, mask);
-  return cudaGetLastError();
-}
-
-cudaError_t resident_worlds_velocity(const ModelDev& m, const DataDev& d, int* worlds) {
-  const TeamShape t = vel_shape(m, d);
-  void (*kern)(ModelDev, DataDev, int);
-  int blocks = 0;
-  cudaError_t e = vel_configured(m, t, &kern);
-  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, 32 * t.wpb, t.block_bytes);
-  *worlds = blocks * t.wpb * (32 / t.lpw);
-  return e;
-}
+size_t smem_velocity(const ModelDev& m, const DataDev& d) { return team_shape(m, d.wn, vel_layout(m).total, vel_kernel).block_bytes; }
+cudaError_t launch_velocity(const ModelDev& m, const DataDev& d, int mask, cudaStream_t s) { return team_launch(m, d, vel_layout(m).total, vel_kernel, mask, s); }
+cudaError_t resident_worlds_velocity(const ModelDev& m, const DataDev& d, int* worlds) { return team_resident_worlds(m, d, vel_layout(m).total, vel_kernel, worlds); }

@@ -15,7 +15,9 @@
 #include <cstdint>
 #include <cuda_runtime.h>
 
+#include "mjb_launch.cuh"
 #include "mjb_math.cuh"
+#include "mjb_types.cuh"
 
 template <int LPW>
 __device__ __forceinline__ float team_sum(float v) {
@@ -106,97 +108,72 @@ struct Stager {
   }
 };
 
-// Per-SM limits of the device, read once per process: SMs, shared memory per SM and the part of it the runtime reserves per
-// block, blocks, warps and registers per SM.  Like the per-instance kernel configuration below, this assumes that the GPUs a
-// process drives are of one kind (one process per GPU, as bench.py and torchrun run it).
-struct SmLimits { int sms; size_t smem_per_sm, reserved_per_block; int blocks, warps, regs; };
-inline const SmLimits& sm_limits() {
-  static const SmLimits l = [] {
-    int dev = 0, sms = 0, smem = 0, reserved = 0, blocks = 0, threads = 0, regs = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaDeviceGetAttribute(&smem, cudaDevAttrMaxSharedMemoryPerMultiprocessor, dev);
-    cudaDeviceGetAttribute(&reserved, cudaDevAttrReservedSharedMemoryPerBlock, dev);
-    cudaDeviceGetAttribute(&blocks, cudaDevAttrMaxBlocksPerMultiprocessor, dev);
-    cudaDeviceGetAttribute(&threads, cudaDevAttrMaxThreadsPerMultiProcessor, dev);
-    cudaDeviceGetAttribute(&regs, cudaDevAttrMaxRegistersPerMultiprocessor, dev);
-    return SmLimits{sms, (size_t)smem, (size_t)reserved, blocks, threads / 32, regs};
-  }();
-  return l;
-}
-
-// Registers per thread of a kernel instance (0 if unknown: then registers do not limit the shape choice).
-template <class K>
-inline int kernel_regs(K* kern) {
-  cudaFuncAttributes a;
-  return cudaFuncGetAttributes(&a, kern) == cudaSuccess ? a.numRegs : 0;
-}
-
-// Shared memory an SM sets aside for a block of `bytes`: 128-byte allocation units plus the runtime's per-block reserve.
-inline size_t sm_block_bytes(size_t bytes) { return ((bytes + 127) & ~(size_t)127) + sm_limits().reserved_per_block; }
-
-// Configuration of a team kernel instance for blocks of `smem` bytes: above the 48 KB default, the block's dynamic shared memory,
-// and the shared-memory carveout (percent of the SM's shared memory) just large enough for as many blocks as fit.  The driver
-// rounds a carveout up to the next shared-memory size the SM supports (CUDA Programming Guide, shared memory of compute
-// capabilities 7.x and later), so the blocks that fit stay resident.  A smaller carveout, which the driver is free to pick
-// otherwise, would cost resident worlds; a larger one costs L1 that the model-table lookups use (three_humanoids k_position,
-// which fits 2 blocks per SM, DESIGN.md §3).  `c` is per instance.
-struct TeamConfig { size_t smem = 0; int carveout = -1; };
-template <class K>
-inline cudaError_t team_configure(K* kern, size_t smem, TeamConfig* c) {
-  const size_t per_sm = sm_limits().smem_per_sm, block = sm_block_bytes(smem), fit = per_sm / block;
-  const size_t pct = fit > 0 ? (100 * fit * block + per_sm - 1) / per_sm : 100;
-  const int carveout = pct < 100 ? (int)pct : (int)cudaSharedmemCarveoutMaxShared;
-  cudaError_t e = cudaSuccess;
-  if (carveout != c->carveout) {
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, carveout);
-    if (e == cudaSuccess) c->carveout = carveout;
-  }
-  if (e == cudaSuccess && smem > 48 * 1024 && smem > c->smem) {
-    e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    if (e == cudaSuccess) c->smem = smem;
-  }
-  return e;
-}
+// ---------------------------------------------------------------- host side: shape, configuration and launch of a team kernel
+// A team kernel (k_position, k_velocity) is one instance per lanes-per-world count, `kernel_of(m, lpw)`, taking (m, d, stage mask),
+// with `world_words` floats of shared memory per world.
+using TeamKernel = void (*)(ModelDev, DataDev, int);
+using TeamChooser = TeamKernel (*)(const ModelDev& m, int lpw);
 
 // Launch shape of a team kernel: lanes per world and warps per block, from the per-world shared-memory footprint.
 // Default 8 lanes per world (4 worlds per warp); models whose worlds are too large for that fall back to fewer worlds per warp.
 // The team kernels are latency bound, so their time is the number of residency rounds (waves of blocks that fit on the SMs at
 // once) times one warp's dependent chain (DESIGN.md §3).  The warps per block (1, 2 or 4) are those that need the fewest rounds
-// for `nworld` worlds, with as many blocks per SM as its shared memory, register file (`regs_of(lpw)`: registers per thread of
-// the kernel instance for lpw), block and warp limits allow; ties go to two-warp blocks.
-struct TeamShape { int lpw, wpb; size_t warp_bytes, block_bytes; };
-template <class F>
-inline TeamShape team_shape(size_t world_words, int nworld, F regs_of) {
+// for `nworld` worlds, with as many blocks per SM as its shared memory, register file (registers per thread of the kernel
+// instance for lpw), block and warp limits allow; ties go to two-warp blocks.  Batched models have only a 32-lane instance:
+// where the footprint alone would give fewer lanes per world, they take 32 lanes in two-warp blocks.
+struct TeamShape { int lpw, wpb; size_t block_bytes; };
+inline TeamShape team_shape(const ModelDev& m, int nworld, size_t world_words, TeamChooser kernel_of) {
   constexpr size_t kBlockMax = 200 * 1024;  // leaves room for a second resident block's reserve
   auto bytes = [&](int lpw) { return (world_words * (size_t)(32 / lpw) + 4) * sizeof(float); };
   int lpw = 8;
   while (lpw < 32 && bytes(lpw) > kBlockMax / 2) lpw *= 2;
   int wpb = 2;
-  const SmLimits& sm = sm_limits();
-  const long groups = (nworld + 32 / lpw - 1) / (32 / lpw);
-  const int warp_regs = (regs_of(lpw) * 32 + 255) & ~255;  // registers are allocated per warp in units of 256
-  auto rounds = [&](int w) {
-    long per_sm = (long)(sm.smem_per_sm / sm_block_bytes(bytes(lpw) * w));
-    per_sm = std::min({per_sm, (long)sm.blocks, (long)(sm.warps / w)});
-    if (warp_regs > 0) per_sm = std::min(per_sm, (long)(sm.regs / warp_regs / w));
-    const long fit = per_sm * sm.sms, blocks = (groups + w - 1) / w;  // fit: blocks resident at once
-    return fit > 0 ? (blocks + fit - 1) / fit : LONG_MAX;
-  };
-  for (int w : {1, 4})
-    if (bytes(lpw) * w <= kBlockMax && rounds(w) < rounds(wpb)) wpb = w;
+  if (m.batched && lpw < 32) {
+    lpw = 32;
+  } else {
+    const SmLimits& sm = sm_limits();
+    const long groups = (nworld + 32 / lpw - 1) / (32 / lpw);
+    const int warp_regs = (kernel_regs(kernel_of(m, lpw)) * 32 + 255) & ~255;  // registers are allocated per warp in units of 256
+    auto rounds = [&](int w) {
+      long per_sm = (long)(sm.smem_per_sm / sm_block_bytes(bytes(lpw) * w));
+      per_sm = std::min({per_sm, (long)sm.blocks, (long)(sm.warps / w)});
+      if (warp_regs > 0) per_sm = std::min(per_sm, (long)(sm.regs / warp_regs / w));
+      const long fit = per_sm * sm.sms, blocks = (groups + w - 1) / w;  // fit: blocks resident at once
+      return fit > 0 ? (blocks + fit - 1) / fit : LONG_MAX;
+    };
+    for (int w : {1, 4})
+      if (bytes(lpw) * w <= kBlockMax && rounds(w) < rounds(wpb)) wpb = w;
+  }
   while (wpb > 1 && bytes(lpw) * wpb > kBlockMax) wpb--;
-  TeamShape t;
-  t.lpw = lpw; t.wpb = wpb; t.warp_bytes = bytes(lpw); t.block_bytes = t.warp_bytes * wpb;
-  return t;
+  return TeamShape{lpw, wpb, bytes(lpw) * wpb};
 }
 
-inline TeamShape team_shape_fixed(size_t world_words, int lpw, int wpb) {
-  TeamShape t;
-  t.lpw = lpw; t.wpb = wpb; t.warp_bytes = (world_words * (size_t)(32 / lpw) + 4) * sizeof(float);
-  while (t.wpb > 1 && t.warp_bytes * t.wpb > 200 * 1024) t.wpb--;
-  t.block_bytes = t.warp_bytes * t.wpb;
-  return t;
+// Shared-memory carveout (percent of the SM's shared memory) for team blocks of `block_bytes`: the one just large enough for as
+// many blocks as fit.  The driver rounds a carveout up to the next shared-memory size the SM supports (CUDA Programming Guide,
+// shared memory of compute capabilities 7.x and later), so the blocks that fit stay resident.  A smaller carveout, which the driver
+// is free to pick otherwise, would cost resident worlds; a larger one costs L1 that the model-table lookups use (three_humanoids
+// k_position, which fits 2 blocks per SM, DESIGN.md §3).
+inline int team_carveout(size_t block_bytes) {
+  const size_t per_sm = sm_limits().smem_per_sm, block = sm_block_bytes(block_bytes), fit = per_sm / block;
+  const size_t pct = fit > 0 ? (100 * fit * block + per_sm - 1) / per_sm : 100;
+  return pct < 100 ? (int)pct : (int)cudaSharedmemCarveoutMaxShared;
+}
+
+inline cudaError_t team_launch(const ModelDev& m, const DataDev& d, size_t world_words, TeamChooser kernel_of, int mask, cudaStream_t s) {
+  const TeamShape t = team_shape(m, d.wn, world_words, kernel_of);
+  const int G = 32 / t.lpw, ngroups = (d.wn + G - 1) / G, grid = (ngroups + t.wpb - 1) / t.wpb;
+  return launch(kernel_of(m, t.lpw), grid, 32 * t.wpb, t.block_bytes, team_carveout(t.block_bytes), s, m, d, mask);
+}
+
+// Worlds per SM resident at once (occupancy API) in the launch shape of d's world range.
+inline cudaError_t team_resident_worlds(const ModelDev& m, const DataDev& d, size_t world_words, TeamChooser kernel_of, int* worlds) {
+  const TeamShape t = team_shape(m, d.wn, world_words, kernel_of);
+  const TeamKernel kern = kernel_of(m, t.lpw);
+  int blocks = 0;
+  cudaError_t e = launch_configure((const void*)kern, t.block_bytes, team_carveout(t.block_bytes));
+  if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, 32 * t.wpb, t.block_bytes);
+  *worlds = blocks * t.wpb * (32 / t.lpw);
+  return e;
 }
 
 // World team of the calling lane.

@@ -150,10 +150,6 @@ enum { STG_KINEMATICS = 1, STG_COM_POS = 2, STG_CAMLIGHT = 4, STG_CRB = 8, STG_T
 enum { STG_VELOCITY = 1, STG_ACTUATION = 2, STG_ACCELERATION = 4, STG_FACTOR_ONLY = 8,
        STG_COMVEL = 16, STG_PASSIVE = 32, STG_RNE = 64 };  // single sub-stages of fwd_velocity (smooth.com_vel, passive.passive, smooth.rne)
 
-// One warp per block: blockIdx.x IS the world, so every world-dependent branch and address is warp-uniform by construction
-// (ptxas keeps them on the uniform datapath and drops the WARPSYNC it otherwise emits around each SHFL).
-constexpr int MJB_WARPS_PER_BLOCK = 1;
-
 // launchers (one per .cu); each returns the cudaError of the launch
 cudaError_t launch_position(const ModelDev& m, const DataDev& d, int stage_mask, cudaStream_t s);
 cudaError_t launch_collision(const ModelDev& m, const DataDev& d, cudaStream_t s);

@@ -180,6 +180,38 @@ def test_g1_replay_matches_oracle(built):
   assert not (d.overflow.cpu().numpy() & ~int(mjw.OverflowType.LS_ITERATIONS)).any()
 
 
+@pytest.mark.parametrize("nworld", [1, 8, 1024])
+def test_g1_step_profile_runs_the_step(built, nworld):
+  """step_profile times the step's own kernel chain (here with the CSR view and the sensors): from the same state it leaves the
+  same qpos / qvel / qacc / sensordata as step, bit for bit, and every one of its six stage groups takes time."""
+  import mujoco_warp_b200 as mjw
+  from mujoco_warp_b200._src.forward import KERNEL_NAMES
+  from mujoco_warp_b200._src.mjcf import MjDataLite
+
+  mjm = mjw.mjcf.load_any(util.G1)
+  mjd = MjDataLite(mjm)
+  ctrls = mjw.load_trajectory(util.G1_TRAJ, mjm, mjd)
+  m = mjw.put_model(mjm)
+  assert m.is_sparse and m.nsensor > 0
+  d = mjw.put_data(mjm, mjd, nworld=nworld, nconmax=48, njmax=192, m=m)
+  jitter = 0.02 * np.random.default_rng(5).uniform(-1, 1, (nworld, mjm.nu))
+  d.ctrl.copy_(torch.from_numpy((ctrls[0][None, :] + jitter).astype(np.float32)))
+  for _ in range(20):  # into contact
+    mjw.step(m, d)
+  state = {n: getattr(d, n).clone() for n in ("qpos", "qvel", "qacc_warmstart", "time")}
+  mjw.step(m, d)
+  torch.cuda.synchronize()
+  want = {n: getattr(d, n).cpu().numpy().copy() for n in ("qpos", "qvel", "qacc", "sensordata")}
+  for n, v in state.items():
+    getattr(d, n).copy_(v)
+  for n in ("qacc", "sensordata"):  # outputs only: what is compared must be what the profiled chain wrote
+    getattr(d, n).fill_(float("nan"))
+  ms = mjw.step_profile(m, d)
+  assert list(ms) == list(KERNEL_NAMES) and all(t > 0 for t in ms.values()), ms
+  for n, v in want.items():
+    np.testing.assert_array_equal(getattr(d, n).cpu().numpy(), v, err_msg=n)
+
+
 # --------------------------------------------------------------------------------------------- mixed-feature scene
 
 
