@@ -26,6 +26,8 @@
  *   mjb_mul_m                  <- _src/support.py:153  mul_m(m, d, res, vec): res = M vec
  *   mjb_sensor_pos/vel/acc     <- _src/sensor.py:810, :1432, :2512  sensor_pos / sensor_vel / sensor_acc(m, d)
  *   mjb_contact_force          <- _src/support.py:445  contact_force(m, d, contact_ids, to_world_frame, force)
+ *   mjb_rays                   <- _src/ray.py:1219 rays(m, d, pnt, vec, geomgroup, flg_static, bodyexclude, dist, geomid, normal) without a
+ *                                 render context (every geom tested, no BVH; no height fields)
  *   mjb_rungekutta4            <- _src/forward.py:523  rungekutta4(m, d)
  *   mjb_solve                  <- _src/solver.py:3671  solve
  *   mjb_euler                  <- _src/forward.py:387  euler (always the semi-implicit Euler update, whatever the model's integrator)
@@ -100,6 +102,12 @@ int mjb_sensor_vel(const mjbModel* m, mjbData* d, void* stream);
 int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream);
 /* support.py:445 contact_force(m, d, contact_ids, to_world_frame, force): force is (n, 6) floats, device pointers */
 int mjb_contact_force(const mjbModel* m, mjbData* d, const int* contact_ids, int n, int to_world_frame, float* force, void* stream);
+/* ray.py:1219 rays: pnt, vec (pnt_nbatch, nray, 3) fp32 device, pnt_nbatch 1 or nworld; geomgroup: 6 host ints (all -1 = no group
+ * filter; NULL = all -1); bodyexclude (nray) int32 device; dist (nworld, nray) fp32, geomid (nworld, nray) int32, normal (nworld, nray, 3)
+ * fp32.  Reads the geom poses of the last kinematics.  A miss gives dist -1, geomid -1 and a zero normal; among equally distant hits the
+ * lowest geom id wins.  One kernel launch (none for nray = 0). */
+int mjb_rays(const mjbModel* m, mjbData* d, const float* pnt, const float* vec, int nray, int pnt_nbatch, const int* geomgroup,
+             int flg_static, const int* bodyexclude, float* dist, int* geomid, float* normal, void* stream);
 /* forward.py:523 rungekutta4(m, d): the integrator alone, after forward() (models compiled with the RK4 integrator) */
 int mjb_rungekutta4(const mjbModel* m, mjbData* d, void* stream);
 int mjb_solve(const mjbModel* m, mjbData* d, void* stream);

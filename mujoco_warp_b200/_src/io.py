@@ -42,7 +42,7 @@ _TENDON_FLOATS = (("tendon_range", 2), ("tendon_margin", 1), ("tendon_stiffness"
                   ("tendon_length0", 1), ("tendon_invweight0", 1), ("tendon_solref_lim", 2), ("tendon_solimp_lim", 5), ("tendon_solref_fri", 2), ("tendon_solimp_fri", 5), ("tendon_actfrcrange", 2))
 # float fields outside _FLOAT_FIELDS that carry the reference's `*` leading dimension as well
 _BATCHABLE_EXTRA = ("eq_solref", "eq_solimp", "eq_data", "pair_friction", "pair_solref", "pair_solreffriction", "pair_solimp", "pair_margin", "pair_gap",
-                    "actuator_dynprm", "actuator_actrange") + tuple(n for n, _ in _TENDON_FLOATS)
+                    "actuator_dynprm", "actuator_actrange", "geom_rgba", "mat_rgba") + tuple(n for n, _ in _TENDON_FLOATS)
 _SIZES = ["nq", "nv", "nu", "na", "nbody", "njnt", "ngeom", "nsite", "ncam", "nlight", "ntree", "nkey", "nmocap", "neq", "ntendon", "nflex"]
 
 _SUPPORTED_PAIRS = {
@@ -500,6 +500,17 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
     setattr(m, n, dev_i(getattr(mjm, n) if nmesh else np.zeros(0)))
   m.mesh_vert = dev_f(np.asarray(mjm.mesh_vert).reshape(-1, 3) if nmesh else np.zeros((0, 3)), batched=False)
   m.mesh_polynormal = dev_f(np.asarray(mjm.mesh_polynormal).reshape(-1, 3) if nmesh else np.zeros((0, 3)), batched=False)
+  # ray casting (reference ray.py:53 _ray_eliminate, :629 ray_mesh): geom visibility, groups and materials, and the mesh triangles.
+  # Models saved before these fields existed get MuJoCo's defaults: opaque grey geoms in group 0, no materials.
+  ng = m.ngeom
+  m.geom_group = dev_i(getattr(mjm, "geom_group", np.zeros(ng)))
+  m.geom_matid = dev_i(getattr(mjm, "geom_matid", -np.ones(ng)))
+  m.geom_rgba = dev_f(np.asarray(getattr(mjm, "geom_rgba", np.tile([0.5, 0.5, 0.5, 1.0], (ng, 1)))).reshape(ng, 4), name="geom_rgba")
+  m.nmat = int(getattr(mjm, "nmat", 0))
+  m.mat_rgba = dev_f(np.asarray(mjm.mat_rgba).reshape(m.nmat, 4) if m.nmat else np.zeros((0, 4)), name="mat_rgba")
+  m.mesh_faceadr = dev_i(getattr(mjm, "mesh_faceadr", np.zeros(nmesh)) if nmesh else np.zeros(0))
+  m.mesh_face = dev_i(np.asarray(getattr(mjm, "mesh_face", np.zeros((0, 3)))).reshape(-1, 3) if nmesh else np.zeros((0, 3)))
+  m.nmeshface = int(m.mesh_face.shape[0])
   m.M_mulm_rowadr, m.M_mulm_col, m.M_mulm_madr = m.mulm_rowadr, m.mulm_col, m.mulm_madr
   anc_pad = np.zeros((m.nbody, m.nv_pad), dtype=np.int32)
   anc_pad[:, : m.nv] = t["body_isdofancestor"]
@@ -519,7 +530,7 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
     iterations=m.opt.iterations, ls_iterations=m.opt.ls_iterations, disableflags=m.opt.disableflags, enableflags=m.opt.enableflags,
     broadphase=int(m.opt.broadphase), broadphase_filter=m.opt.broadphase_filter, qld_total=t["qld_total"], maxtree=t["maxtree"],
     has_multicontact_geom=int(np.isin(_np(mjm, "geom_type"), (C.GEOM_ELLIPSOID, C.GEOM_CYLINDER, C.GEOM_BOX, C.GEOM_MESH)).any()), nmesh=nmesh, na=m.na, ntendon=m.ntendon, nJten=m.nJten, ntenfric=m.ntenfric, nwrap=m.nwrap,
-    nmocap=int(getattr(mjm, "nmocap", 0)), npair=npair, has_convex_pair=t["has_convex_pair"], ccd_iterations=int(getattr(o, "ccd_iterations", 35)), epa_iterations=t["epa_iterations"], nsensor=m.nsensor, nsensordata=m.nsensordata, sensor_subtree_vel=int(m.sensor_subtree_vel), sensor_rne_postconstraint=int(m.sensor_rne_postconstraint), neq=neq, nlimit_ball=len(t["jnt_limited_ball_adr"]), has_gravcomp=int((np.asarray(mjm.body_gravcomp) != 0).any() or (np.asarray(mjm.jnt_stiffness)[np.isin(np.asarray(mjm.jnt_type), (C.JNT_FREE, C.JNT_BALL))] != 0).any()),
+    nmocap=int(getattr(mjm, "nmocap", 0)), npair=npair, has_convex_pair=t["has_convex_pair"], ccd_iterations=int(getattr(o, "ccd_iterations", 35)), epa_iterations=t["epa_iterations"], nsensor=m.nsensor, nsensordata=m.nsensordata, nmat=m.nmat, nmeshface=m.nmeshface, sensor_subtree_vel=int(m.sensor_subtree_vel), sensor_rne_postconstraint=int(m.sensor_rne_postconstraint), neq=neq, nlimit_ball=len(t["jnt_limited_ball_adr"]), has_gravcomp=int((np.asarray(mjm.body_gravcomp) != 0).any() or (np.asarray(mjm.jnt_stiffness)[np.isin(np.asarray(mjm.jnt_type), (C.JNT_FREE, C.JNT_BALL))] != 0).any()),
   )
   for k, v in ints.items():
     _lib.check(L.mjb_model_set_int(h, k.encode(), int(v)))
@@ -541,7 +552,8 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
                                          "mesh_polynum", "mesh_polyadr", "mesh_polyvertadr", "mesh_polyvertnum", "mesh_polyvert", "mesh_polymapadr", "mesh_polymapnum",
                                          "mesh_polymap", "mesh_vert", "mesh_polynormal", "actuator_dyntype", "actuator_actadr", "actuator_actnum",
                                          "actuator_actlimited", "actuator_actearly", "actuator_dynprm", "actuator_actrange", "actuator_trntype",
-                                         "ten_J_rownnz", "ten_J_rowadr", "ten_J_colind", "tendon_adr", "tendon_num", "wrap_objid", "tendon_limited", "tendon_actfrclimited", "wrap_prm", "ten_J0"]
+                                         "ten_J_rownnz", "ten_J_rowadr", "ten_J_colind", "tendon_adr", "tendon_num", "wrap_objid", "tendon_limited", "tendon_actfrclimited", "wrap_prm", "ten_J0",
+                                         "geom_group", "geom_matid", "geom_rgba", "mat_rgba", "mesh_faceadr", "mesh_face"]
                                         + [n for n, _ in _TENDON_FLOATS]):
     dev_names.setdefault(n, getattr(m, n))
   for n, x in dev_names.items():

@@ -624,6 +624,16 @@ def compile_xml(root):
       meshes.append(_mesh.process(_vec(me.get("vertex")).reshape(-1, 3), None if ma.get("inertia") == "convex" else faces, _vec(ma.get("scale"), 3, default=[1, 1, 1])))
       mesh_names.append(me.get("name", f"mesh{len(mesh_names)}"))
 
+  # materials: only the colour is compiled (a fully transparent material hides its geoms from rays); every other material and
+  # texture attribute is ignored
+  mat_names, mat_rgba = [], []
+  for asset in root.findall("asset"):
+    for me in asset.findall("material"):
+      ma = dflt.resolve("material", me.get("class", "main"))
+      ma.update(me.attrib)
+      mat_names.append(me.get("name", f"material{len(mat_names)}"))
+      mat_rgba.append(_vec(ma.get("rgba"), 4, default=[1, 1, 1, 1]))
+
   def attrs(elem, childclass):
     cls = elem.get("class", childclass)
     out = dflt.resolve(elem.tag, cls if cls is not None else "main")
@@ -765,6 +775,8 @@ def compile_xml(root):
           density=float(a.get("density", 1000.0)),
           mass=float(a["mass"]) if "mass" in a else None,
           group=int(a.get("group", 0)),
+          rgba=_vec(a.get("rgba"), 4, default=[0.5, 0.5, 0.5, 1.0]),
+          matid=mat_names.index(a["material"]) if a.get("material") in mat_names else -1,
           dataid=dataid,
         )
         if b["geomnum"] == 0:
@@ -978,6 +990,12 @@ def compile_xml(root):
   m.geom_condim = np.array([g["condim"] for g in geoms], dtype=np.int32)
   m.geom_priority = np.array([g["priority"] for g in geoms], dtype=np.int32)
   m.geom_dataid = np.array([g["dataid"] for g in geoms], dtype=np.int32).reshape(ngeom)
+  m.geom_group = np.array([g["group"] for g in geoms], dtype=np.int32).reshape(ngeom)
+  m.geom_matid = np.array([g["matid"] for g in geoms], dtype=np.int32).reshape(ngeom)
+  m.geom_rgba = np.array([g["rgba"] for g in geoms]).reshape(ngeom, 4)
+  m.nmat = len(mat_names)
+  m.mat_rgba = np.array(mat_rgba).reshape(m.nmat, 4)
+  m.names.material = list(mat_names)
   m.geom_size = np.array([g["size"] for g in geoms]).reshape(ngeom, 3)
   m.geom_pos = np.array([g["pos"] for g in geoms]).reshape(ngeom, 3)
   m.geom_quat = np.array([g["quat"] for g in geoms]).reshape(ngeom, 4)

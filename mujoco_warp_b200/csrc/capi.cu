@@ -214,6 +214,17 @@ int mjb_contact_force(const mjbModel* m, mjbData* d, const int* contact_ids, int
   MJB_LAUNCH(launch_contact_force(m->dev, d->dev, contact_ids, n, to_world_frame, force, s));
   return 0;
 }
+int mjb_rays(const mjbModel* m, mjbData* d, const float* pnt, const float* vec, int nray, int pnt_nbatch, const int* geomgroup, int flg_static,
+             const int* bodyexclude, float* dist, int* geomid, float* normal, void* stream) {
+  MJB_ENTER();
+  const int nworld = d->dev.nworld;
+  if (nray < 0) return fail("mjb_rays: nray must be >= 0, got " + std::to_string(nray));
+  if (pnt_nbatch != 1 && pnt_nbatch != nworld) return fail("mjb_rays: pnt_nbatch must be 1 or nworld (" + std::to_string(nworld) + "), got " + std::to_string(pnt_nbatch));
+  if ((long long)nworld * nray > 0x7fffffffLL) return fail("mjb_rays: nworld * nray exceeds the int range");
+  if (nray > 0 && (!pnt || !vec || !bodyexclude || !dist || !geomid || !normal)) return fail("mjb_rays: null array");
+  MJB_LAUNCH(launch_ray(m->dev, d->dev, pnt, vec, nray, pnt_nbatch, geomgroup, flg_static, bodyexclude, dist, geomid, normal, s));
+  return 0;
+}
 int mjb_sensor_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 1, s)); return 0; }
 int mjb_sensor_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 2, s)); return 0; }
 int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 4, s)); return 0; }

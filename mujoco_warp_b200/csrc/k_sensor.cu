@@ -8,6 +8,7 @@
 // the solver evaluates all three stages (the stage mask lets sensor_pos / sensor_vel / sensor_acc be called on their own).
 #include "mjb_launch.cuh"
 #include "mjb_math.cuh"
+#include "mjb_ray.cuh"
 #include "mjb_types.cuh"
 
 namespace {
@@ -36,84 +37,6 @@ __device__ __forceinline__ const float* obj_mat(const DataDev& d, const ModelDev
     case OBJ_SITE: return d.site_xmat + (wb * m.nsite + id) * 9;
     default: return d.cam_xmat + (wb * m.ncam + id) * 9;
   }
-}
-
-// ray.py:106 _ray_quad: smallest non-negative root of a x^2 + 2 b x + c = 0 (both roots in x2), -1 if none
-__device__ float ray_quad(float a, float b, float c, float* x2) {
-  float det = b * b - a * c;
-  x2[0] = x2[1] = -1.f;
-  if (det < MJ_MINVAL) return -1.f;
-  det = sqrtf(det);
-  const float den = a != 0.f ? 1.0f / a : 0.f;
-  x2[0] = (-b - det) * den; x2[1] = (-b + det) * den;
-  return x2[0] >= 0.f ? x2[0] : (x2[1] >= 0.f ? x2[1] : -1.f);
-}
-__device__ float ray_sphere(v3 pos, float dist_sqr, v3 pnt, v3 vec) {  // ray.py:238
-  const v3 dif = pnt - pos;
-  float xx[2];
-  return ray_quad(dot(vec, vec), dot(vec, dif), dot(dif, dif) - dist_sqr, xx);
-}
-// ray.py:799 ray_geom, distance only, for the shapes a site can have
-__device__ float ray_geom_dist(v3 pos, const float* mat, v3 size, v3 pnt, v3 vec, int type) {
-  float xx[2];
-  if (type == GEOM_SPHERE) return ray_sphere(pos, size.x * size.x, pnt, vec);
-  const v3 lpnt = mat_t_vec(mat, pnt - pos), lvec = mat_t_vec(mat, vec);  // :33 _ray_map
-  if (type == GEOM_CAPSULE) {  // :255
-    const float ssz = size.x + size.y;
-    if (ray_sphere(pos, ssz * ssz, pnt, vec) < 0.f) return -1.f;
-    float x = -1.f;
-    const float sq = size.x * size.x;
-    float a = lvec.x * lvec.x + lvec.y * lvec.y, b = lvec.x * lpnt.x + lvec.y * lpnt.y, c = lpnt.x * lpnt.x + lpnt.y * lpnt.y - sq;
-    const float sol = ray_quad(a, b, c, xx);
-    if (sol >= 0.f && fabsf(lpnt.z + sol * lvec.z) <= size.y) if (x < 0.f || sol < x) x = sol;
-    v3 ldif = mk3(lpnt.x, lpnt.y, lpnt.z - size.y);
-    a += lvec.z * lvec.z; b = dot(lvec, ldif); c = dot(ldif, ldif) - sq;
-    ray_quad(a, b, c, xx);
-    for (int i = 0; i < 2; i++) if (xx[i] >= 0.f && lpnt.z + xx[i] * lvec.z >= size.y) if (x < 0.f || xx[i] < x) x = xx[i];
-    ldif.z = lpnt.z + size.y;
-    b = dot(lvec, ldif); c = dot(ldif, ldif) - sq;
-    ray_quad(a, b, c, xx);
-    for (int i = 0; i < 2; i++) if (xx[i] >= 0.f && lpnt.z + xx[i] * lvec.z <= -size.y) if (x < 0.f || xx[i] < x) x = xx[i];
-    return x;
-  }
-  if (type == GEOM_ELLIPSOID) {  // :329
-    const v3 si = mk3(size.x != 0.f ? 1.0f / (size.x * size.x) : 0.f, size.y != 0.f ? 1.0f / (size.y * size.y) : 0.f, size.z != 0.f ? 1.0f / (size.z * size.z) : 0.f);
-    const v3 sv = mk3(si.x * lvec.x, si.y * lvec.y, si.z * lvec.z), sp = mk3(si.x * lpnt.x, si.y * lpnt.y, si.z * lpnt.z);
-    return ray_quad(dot(sv, lvec), dot(sv, lpnt), dot(sp, lpnt) - 1.0f, xx);
-  }
-  if (type == GEOM_CYLINDER) {  // :360
-    if (ray_sphere(pos, size.x * size.x + size.y * size.y, pnt, vec) < 0.f) return -1.f;
-    float x = -1.f;
-    if (fabsf(lvec.z) > MJ_MINVAL)
-      for (int side = -1; side <= 1; side += 2) {
-        const float sol = ((float)side * size.y - lpnt.z) / lvec.z;
-        if (sol >= 0.f) {
-          const float p0 = lpnt.x + sol * lvec.x, p1 = lpnt.y + sol * lvec.y;
-          if (p0 * p0 + p1 * p1 <= size.x * size.x) if (x < 0.f || sol < x) x = sol;
-        }
-      }
-    const float a = lvec.x * lvec.x + lvec.y * lvec.y, b = lvec.x * lpnt.x + lvec.y * lpnt.y, c = lpnt.x * lpnt.x + lpnt.y * lpnt.y - size.x * size.x;
-    const float sol = ray_quad(a, b, c, xx);
-    if (sol >= 0.f && fabsf(lpnt.z + sol * lvec.z) <= size.y) if (x < 0.f || sol < x) x = sol;
-    return x;
-  }
-  if (type == GEOM_BOX) {  // :421
-    if (ray_sphere(pos, dot(size, size), pnt, vec) < 0.f) return -1.f;
-    float x = -1.f;
-    for (int i = 0; i < 3; i++) {
-      const float lv = comp3(lvec, i);
-      if (fabsf(lv) <= MJ_MINVAL) continue;
-      for (int side = -1; side <= 1; side += 2) {
-        const float sol = ((float)side * comp3(size, i) - comp3(lpnt, i)) / lv;
-        if (sol < 0.f) continue;
-        const int id0 = i == 0 ? 1 : 0, id1 = i == 2 ? 1 : 2;
-        const float p0 = comp3(lpnt, id0) + sol * comp3(lvec, id0), p1 = comp3(lpnt, id1) + sol * comp3(lvec, id1);
-        if (fabsf(p0) <= comp3(size, id0) && fabsf(p1) <= comp3(size, id1)) if (x < 0.f || sol < x) x = sol;
-      }
-    }
-    return x;
-  }
-  return -1.f;
 }
 
 __device__ __forceinline__ int obj_body(const ModelDev& m, int objtype, int id) {  // sensor.py:1066 / :320
@@ -406,8 +329,8 @@ k_sensor(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d,
           if (nf <= 0.f) continue;
           v3 ray = normalize(ld3(d.contact_frame + 9 * (size_t)c) * nf);
           if (body == b2) ray = ray * -1.0f;
-          if (ray_geom_dist(ld3(d.site_xpos + (wb * m.nsite + id) * 3), d.site_xmat + (wb * m.nsite + id) * 9, ld3(m.site_size + 3 * id),
-                            ld3(d.contact_pos + 3 * (size_t)c), ray, m.site_type[id]) >= 0.f) total += nf;
+          if (ray_geom<false>(ld3(d.site_xpos + (wb * m.nsite + id) * 3), d.site_xmat + (wb * m.nsite + id) * 9, ld3(m.site_size + 3 * id),
+                              ld3(d.contact_pos + 3 * (size_t)c), ray, m.site_type[id], nullptr) >= 0.f) total += nf;
         }
         v[0] = total; break; }
       case SENS_FORCE: {  // sensor.py:1542

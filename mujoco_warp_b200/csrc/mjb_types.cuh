@@ -8,7 +8,7 @@
 #define MJB_MODEL_INTS(X) \
   X(nq) X(nv) X(nu) X(nbody) X(njnt) X(ngeom) X(nsite) X(ncam) X(nlight) X(nC) X(ntree) X(nJmom) X(nlevel) \
   X(nxn_npair) X(nlimit) X(nfricdof) X(nmaxpyramid) X(integrator) X(cone) X(solver) X(iterations) \
-  X(ls_iterations) X(disableflags) X(enableflags) X(broadphase) X(broadphase_filter) X(qld_total) X(maxtree) X(has_multicontact_geom) X(neq) X(nlimit_ball) X(has_gravcomp) X(nmocap) X(npair) X(has_convex_pair) X(ccd_iterations) X(epa_iterations) X(nsensor) X(nsensordata) X(sensor_subtree_vel) X(sensor_rne_postconstraint) X(nmesh) X(na) X(ntendon) X(nJten) X(ntenfric) X(nwrap)
+  X(ls_iterations) X(disableflags) X(enableflags) X(broadphase) X(broadphase_filter) X(qld_total) X(maxtree) X(has_multicontact_geom) X(neq) X(nlimit_ball) X(has_gravcomp) X(nmocap) X(npair) X(has_convex_pair) X(ccd_iterations) X(epa_iterations) X(nsensor) X(nsensordata) X(sensor_subtree_vel) X(sensor_rne_postconstraint) X(nmesh) X(na) X(ntendon) X(nJten) X(ntenfric) X(nwrap) X(nmat) X(nmeshface)
 #define MJB_MODEL_FLOATS(X) \
   X(timestep) X(tolerance) X(ls_tolerance) X(impratio_invsqrt) X(meaninertia) X(gravity_x) X(gravity_y) X(gravity_z) X(ccd_tolerance)
 #define MJB_MODEL_IARRS(X) \
@@ -26,7 +26,7 @@
   X(nxn_geom_pair) X(nxn_pairid) X(body_isdofancestor) X(eq_type) X(eq_obj1id) X(eq_obj2id) X(jnt_limited_ball_adr) X(pair_dim) \
   X(sensor_type) X(sensor_datatype) X(sensor_needstage) X(sensor_objtype) X(sensor_objid) X(sensor_reftype) X(sensor_refid) X(sensor_dim) X(sensor_adr) X(site_type) \
   X(geom_dataid) X(mesh_vertadr) X(mesh_vertnum) X(mesh_graphadr) X(mesh_graph) X(mesh_polynum) X(mesh_polyadr) X(mesh_polyvertadr) X(mesh_polyvertnum) \
-  X(mesh_polyvert) X(mesh_polymapadr) X(mesh_polymapnum) X(mesh_polymap)
+  X(mesh_polyvert) X(mesh_polymapadr) X(mesh_polymapnum) X(mesh_polymap) X(geom_group) X(geom_matid) X(mesh_faceadr) X(mesh_face)
 #define MJB_MODEL_FARRS(X) \
   X(qpos0) X(qpos_spring) X(body_pos) X(body_quat) X(body_ipos) X(body_iquat) X(body_mass) X(body_subtreemass) \
   X(body_inertia) X(body_invweight0) X(body_gravcomp) X(jnt_pos) X(jnt_axis) X(jnt_stiffness) X(jnt_range) X(jnt_margin) X(jnt_solref) \
@@ -38,7 +38,8 @@
   X(eq_solref) X(eq_solimp) X(eq_data) X(pair_friction) X(pair_solref) X(pair_solreffriction) X(pair_solimp) X(pair_margin) X(pair_gap) \
   X(sensor_cutoff) X(site_size) X(mesh_vert) X(mesh_polynormal) X(actuator_dynprm) X(actuator_actrange) \
   X(wrap_prm) X(ten_J0) X(tendon_range) X(tendon_margin) X(tendon_stiffness) X(tendon_damping) X(tendon_frictionloss) X(tendon_lengthspring) \
-  X(tendon_length0) X(tendon_invweight0) X(tendon_solref_lim) X(tendon_solimp_lim) X(tendon_solref_fri) X(tendon_solimp_fri) X(tendon_actfrcrange)
+  X(tendon_length0) X(tendon_invweight0) X(tendon_solref_lim) X(tendon_solimp_lim) X(tendon_solref_fri) X(tendon_solimp_fri) X(tendon_actfrcrange) \
+  X(geom_rgba) X(mat_rgba)
 
 struct ModelDev {
 #define X(n) int n;
@@ -168,6 +169,9 @@ size_t smem_implicit(const ModelDev& m);
 cudaError_t launch_sensor(const ModelDev& m, const DataDev& d, int stages, cudaStream_t s);
 cudaError_t launch_contact_force(const ModelDev& m, const DataDev& d, const int* contact_ids, int n, int to_world, float* out, cudaStream_t s);
 cudaError_t launch_rk_stage(const ModelDev& m, const DataDev& d, float* rk, int stage, cudaStream_t s);
+// rays (nworld x nray, world-major) against every geom of every world; geomgroup: 6 ints, all -1 = no group filter (k_ray.cu)
+cudaError_t launch_ray(const ModelDev& m, const DataDev& d, const float* pnt, const float* vec, int nray, int pnt_nbatch, const int* geomgroup, int flg_static,
+                       const int* bodyexclude, float* dist, int* geomid, float* normal, cudaStream_t s);
 cudaError_t launch_ctrl_noise(const ModelDev& m, const DataDev& d, const float* ctrl_center, int step, float std, float rate, cudaStream_t s);
 size_t smem_position(const ModelDev& m, const DataDev& d);
 size_t smem_collision(const ModelDev& m, const DataDev& d);

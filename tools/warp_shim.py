@@ -675,6 +675,7 @@ def _install_runtime(wp):
       return Tile
 
   wp.tile = _TileCtor()
+  wp.tile_argmin = lambda t: [int(_np.argmin(t.a))]  # index of the first minimum (ray.py:995)
   wp.tile_extract = lambda t, *i: t[i if len(i) > 1 else i[0]]
 
   def _sym(a, fill_mode):
