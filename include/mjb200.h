@@ -7,6 +7,8 @@
  *                                 the reference binds wp.array pointers into wp.launch argument lists)
  *   mjb_step                   <- _src/forward.py:1368 step(m, d)
  *   mjb_forward                <- _src/forward.py:1341 forward(m, d)
+ *   mjb_inverse                <- _src/inverse.py:148  inverse(m, d): position and velocity stages, then the constraint forces at the
+ *                                                      given d.qacc and qfrc_inverse; ENBL_INVDISCRETE converts a discrete-time qacc first
  *   mjb_fwd_position           <- _src/forward.py:635  fwd_position(m, d, factorize=False)
  *   mjb_kinematics             <- _src/smooth.py:447   kinematics
  *   mjb_com_pos                <- _src/smooth.py:824   com_pos
@@ -78,6 +80,11 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m);
 /* ---- pipeline */
 int mjb_step(const mjbModel* m, mjbData* d, void* stream);
 int mjb_forward(const mjbModel* m, mjbData* d, void* stream);
+/* inverse.py:148 inverse: fwd_position and fwd_velocity (with actuation and the factor of M, as forward), then at the given d.qacc:
+ * efc_force / efc_state / efc_Ma, qfrc_constraint, solver_niter = 0, qfrc_inverse = qfrc_bias + M qacc - qfrc_passive - qfrc_constraint,
+ * and the sensors.  With ENBL_INVDISCRETE (Euler unless eulerdamp is disabled, implicitfast) d.qacc is a discrete-time acceleration:
+ * everything above uses its continuous-time counterpart, and d.qacc is left as it was.  Error for RK4 / implicit with ENBL_INVDISCRETE. */
+int mjb_inverse(const mjbModel* m, mjbData* d, void* stream);
 int mjb_fwd_position(const mjbModel* m, mjbData* d, void* stream);
 int mjb_kinematics(const mjbModel* m, mjbData* d, void* stream);
 int mjb_com_pos(const mjbModel* m, mjbData* d, void* stream);

@@ -297,10 +297,10 @@ def _validate(mjm):
     raise NotImplementedError("fluid forces (opt.density / viscosity / wind) are not implemented")
   if int(getattr(o, "noslip_iterations", 0)) > 0:
     raise NotImplementedError("the noslip solver (opt.noslip_iterations > 0) is not implemented")
-  unsupported_enable = int(o.enableflags) & (C.ENBL_OVERRIDE | C.ENBL_ENERGY | C.ENBL_FWDINV | C.ENBL_INVDISCRETE | C.ENBL_SLEEP)
+  unsupported_enable = int(o.enableflags) & (C.ENBL_OVERRIDE | C.ENBL_ENERGY | C.ENBL_FWDINV | C.ENBL_SLEEP)
   if unsupported_enable:
     names = [n for n, b in C.ENABLE_FLAGS.items() if unsupported_enable & b]
-    raise NotImplementedError(f"enable flag(s) {names} are not implemented (contact override, energy, fwdinv / invdiscrete, sleeping)")
+    raise NotImplementedError(f"enable flag(s) {names} are not implemented (contact override, energy, fwdinv, sleeping)")
   if getattr(mjm, "nu", 0):
     gt, bt = np.asarray(mjm.actuator_gaintype), np.asarray(mjm.actuator_biastype)
     if not np.isin(gt, (C.GAIN_FIXED, C.GAIN_AFFINE)).all():
@@ -695,7 +695,7 @@ _BOUND_TOP = [
   "time", "qpos", "qvel", "ctrl", "qacc_warmstart", "qfrc_applied", "xfrc_applied", "qacc", "xpos", "xquat", "xmat", "xipos", "ximat", "xanchor",
   "xaxis", "geom_xpos", "geom_xmat", "site_xpos", "site_xmat", "cam_xpos", "cam_xmat", "light_xpos", "light_xdir", "subtree_com", "cdof", "cinert",
   "crb", "M", "qLD", "actuator_length", "actuator_moment", "actuator_velocity", "cvel", "cdof_dot", "qfrc_bias", "qfrc_spring", "qfrc_damper",
-  "qfrc_gravcomp", "qfrc_passive", "actuator_force", "qfrc_actuator", "qfrc_smooth", "qacc_smooth", "qfrc_constraint", "cacc", "cfrc_int",
+  "qfrc_gravcomp", "qfrc_passive", "actuator_force", "qfrc_actuator", "qfrc_smooth", "qacc_smooth", "qfrc_constraint", "qfrc_inverse", "cacc", "cfrc_int",
   "ne", "nf", "nl", "nefc", "nacon", "ncollision", "solver_niter", "overflow", "moment_rownnz", "moment_rowadr", "moment_colind", "eq_active", "mocap_pos", "mocap_quat", "sensordata", "subtree_linvel", "subtree_angmom", "cfrc_ext",
   "act", "act_dot", "ten_length", "ten_J", "ten_velocity", "qLU",
 ]

@@ -23,6 +23,9 @@ struct mjbData {
   cudaEvent_t ev_fork, ev_join[8];
   int nsplit;
   float* rk;  // Runge-Kutta scratch, (nworld, nq + 3 nv + 2 na); allocated by mjb_data_finalize for RK4 models only
+  // inverse dynamics (k_inverse.cu takes them as arguments: DataDev stays as the other kernels know it)
+  float* qfrc_inverse;  // Data.qfrc_inverse, (nworld, nv), bound by name like the DataDev arrays
+  float* inv_qacc;      // (nworld, nv) continuous-time acceleration of discrete inverse dynamics, read by its sensor launch
 };
 
 namespace {
@@ -103,6 +106,8 @@ mjbData* mjb_data_create(int nworld, int nconmax, int naconmax, int njmax, int n
   d->finalized = false;
   d->nsplit = 1;
   d->rk = nullptr;
+  d->qfrc_inverse = nullptr;
+  d->inv_qacc = nullptr;
   return d;
 }
 void mjb_data_destroy(mjbData* d) {
@@ -110,6 +115,7 @@ void mjb_data_destroy(mjbData* d) {
   if (d->dev.world_conadr) cudaFree(d->dev.world_conadr);
   if (d->dev.world_ncon) cudaFree(d->dev.world_ncon);
   if (d->dev.imp_qacc) cudaFree(d->dev.imp_qacc);
+  if (d->inv_qacc) cudaFree(d->inv_qacc);
   if (d->rk) cudaFree(d->rk);
   if (d->nsplit > 1) {
     for (int i = 0; i < d->nsplit; i++) { cudaStreamDestroy(d->aux[i]); cudaEventDestroy(d->ev_join[i]); }
@@ -122,6 +128,7 @@ int mjb_data_set_int(mjbData* d, const char* name, int v) {
   return fail(std::string("unknown data int field: ") + name);
 }
 int mjb_data_set_array(mjbData* d, const char* name, void* p) {
+  if (!strcmp(name, "qfrc_inverse")) { d->qfrc_inverse = (float*)p; return 0; }
 #define X(n) if (!strcmp(name, #n)) { d->dev.n = (float*)p; return 0; }
   MJB_DATA_FARRS(X)
 #undef X
@@ -136,6 +143,7 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
   MJB_DATA_FARRS(X)
   MJB_DATA_IARRS(X)
 #undef X
+  if (!d->qfrc_inverse) return fail("data array not set: qfrc_inverse");
   if (d->dev.nv_pad < m->dev.nv) return fail("nv_pad < nv");
   if (check(cudaMalloc(&d->dev.world_conadr, sizeof(int) * (size_t)d->dev.nworld), "cudaMalloc(world_conadr)")) return -1;
   if (check(cudaMalloc(&d->dev.world_ncon, sizeof(int) * (size_t)d->dev.nworld), "cudaMalloc(world_ncon)")) return -1;
@@ -143,6 +151,8 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
   if (check(cudaMemset(d->dev.world_ncon, 0, sizeof(int) * (size_t)d->dev.nworld), "memset")) return -1;
   // always there (nworld x nv floats), so that switching Option.integrator to the fully implicit one needs no allocation inside a graph capture
   if (check(cudaMalloc(&d->dev.imp_qacc, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nv > 0 ? m->dev.nv : 1)), "cudaMalloc(imp_qacc)")) return -1;
+  // likewise always there, so that enabling discrete inverse dynamics (Option.enableflags) needs no allocation either
+  if (!d->inv_qacc && check(cudaMalloc(&d->inv_qacc, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nv > 0 ? m->dev.nv : 1)), "cudaMalloc(inv_qacc)")) return -1;
   if (m->dev.integrator == INT_RK4 && !d->rk &&
       check(cudaMalloc(&d->rk, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nq + 3 * m->dev.nv + 2 * m->dev.na + 1)), "cudaMalloc(rk)")) return -1;
   const size_t smem[6] = {smem_position(m->dev, d->dev), smem_collision(m->dev, d->dev), smem_constraint(m->dev, d->dev),
@@ -232,12 +242,18 @@ int mjb_solve(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LA
 int mjb_euler(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_integrate(m->dev, d->dev, INT_EULER, s)); return 0; }
 
 // which stages a pipeline call runs
-enum { RUN_POSITION = 1, RUN_VELOCITY = 2, RUN_SOLVER = 4, RUN_EULER = 8 };
+enum { RUN_POSITION = 1, RUN_VELOCITY = 2, RUN_SOLVER = 4, RUN_EULER = 8, RUN_INVERSE = 16 };
+
+// inverse.py:79-119 discrete_acc: whether the given qacc is converted from discrete time (Euler without eulerdamp=disable, implicitfast)
+static bool inverse_discrete(const ModelDev& m) {
+  if (!(m.enableflags & ENBL_INVDISCRETE)) return false;
+  return m.integrator == INT_IMPLICITFAST || (m.integrator == INT_EULER && !(m.disableflags & DSBL_EULERDAMP));
+}
 
 // The kernels of the stages in `what` for dd's world range.  With `marks` (six events), the end of each stage group is recorded
 // in the order of forward.KERNEL_NAMES: position, collision, constraint (with the CSR view), velocity, solver (with the sensors),
 // integrate (every integrator kernel).
-static int chain(const mjbModel* m, const DataDev& dd, int what, cudaStream_t s, cudaEvent_t* marks = nullptr) {
+static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int what, cudaStream_t s, cudaEvent_t* marks = nullptr) {
 #define MJB_MARK(i) do { if (marks && check(cudaEventRecord(marks[i], s), "cudaEventRecord")) return -1; } while (0)
   if (what & RUN_POSITION) {
     // forward.py:635-677 with factorize=False: kinematics, com_pos, camlight, crb, collision, make_constraint, transmission
@@ -259,6 +275,17 @@ static int chain(const mjbModel* m, const DataDev& dd, int what, cudaStream_t s,
     if (m->dev.nsensor > 0) MJB_LAUNCH(launch_sensor(m->dev, dd, 7, s));
     MJB_MARK(4);
   }
+  if (what & RUN_INVERSE) {
+    // inverse dynamics at the given qacc, then the sensors of all three stages; with a discrete-time qacc they read the continuous
+    // one k_inverse wrote to the scratch, and d.qacc itself is never written
+    const bool disc = inverse_discrete(m->dev);
+    MJB_LAUNCH(launch_inverse(m->dev, dd, d->qfrc_inverse, d->inv_qacc, disc, s));
+    if (m->dev.nsensor > 0) {
+      DataDev ds = dd;
+      if (disc) ds.qacc = d->inv_qacc;
+      MJB_LAUNCH(launch_sensor(m->dev, ds, 7, s));
+    }
+  }
   if (what & RUN_EULER) {
     if (m->dev.integrator == INT_IMPLICIT && smem_implicit(m->dev) > kMaxSmem) return fail("implicit integrator: the velocity-derivative scratch (18 x nbody x 32 floats) exceeds one block's shared memory");
     MJB_LAUNCH(launch_integrate(m->dev, dd, -1, s));
@@ -271,12 +298,12 @@ static int chain(const mjbModel* m, const DataDev& dd, int what, cudaStream_t s,
 int mjb_implicit(const mjbModel* m, mjbData* d, void* stream) {
   MJB_ENTER();
   if (m->dev.integrator != INT_IMPLICIT && m->dev.integrator != INT_IMPLICITFAST) return fail("mjb_implicit: the model's integrator is Euler / RK4 (the factor-and-solve scratch is sized by the integrator the model was created with)");
-  return chain(m, d->dev, RUN_EULER, s);
+  return chain(m, d, d->dev, RUN_EULER, s);
 }
 
 static int pipeline(const mjbModel* m, mjbData* d, int what, cudaStream_t s) {
   if (what & RUN_POSITION) MJB_LAUNCH(reset_contact_counters(d->dev, s));
-  if (d->nsplit < 2) return chain(m, d->dev, what, s);
+  if (d->nsplit < 2) return chain(m, d, d->dev, what, s);
   // fork: both halves wait for everything queued on the caller's stream, run their own kernel chain, and are joined back
   if (check(cudaEventRecord(d->ev_fork, s), "cudaEventRecord")) return -1;
   const int part = (d->dev.nworld + d->nsplit - 1) / d->nsplit;
@@ -286,7 +313,7 @@ static int pipeline(const mjbModel* m, mjbData* d, int what, cudaStream_t s) {
     dd.wn = min(part, d->dev.nworld - dd.w0);
     if (dd.wn <= 0) break;
     if (check(cudaStreamWaitEvent(d->aux[h], d->ev_fork, 0), "cudaStreamWaitEvent")) return -1;
-    if (chain(m, dd, what, d->aux[h])) return -1;
+    if (chain(m, d, dd, what, d->aux[h])) return -1;
     if (check(cudaEventRecord(d->ev_join[h], d->aux[h]), "cudaEventRecord")) return -1;
     if (check(cudaStreamWaitEvent(s, d->ev_join[h], 0), "cudaStreamWaitEvent")) return -1;
   }
@@ -294,6 +321,12 @@ static int pipeline(const mjbModel* m, mjbData* d, int what, cudaStream_t s) {
 }
 int mjb_fwd_position(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); return pipeline(m, d, RUN_POSITION, s); }
 int mjb_forward(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); return pipeline(m, d, RUN_POSITION | RUN_VELOCITY | RUN_SOLVER, s); }
+int mjb_inverse(const mjbModel* m, mjbData* d, void* stream) {
+  MJB_ENTER();
+  if ((m->dev.enableflags & ENBL_INVDISCRETE) && (m->dev.integrator == INT_RK4 || m->dev.integrator == INT_IMPLICIT))
+    return fail("mjb_inverse: discrete inverse dynamics (ENBL_INVDISCRETE) is not supported for the RK4 and implicit integrators");
+  return pipeline(m, d, RUN_POSITION | RUN_VELOCITY | RUN_INVERSE, s);
+}
 // forward.py:523-555 rungekutta4, called after forward(): three more forward() evaluations with the state bookkeeping in between
 static int rk4_after_forward(const mjbModel* m, mjbData* d, cudaStream_t s) {
   if (!d->rk) return fail("Runge-Kutta scratch missing: data was finalized against a model whose integrator is not RK4");
@@ -320,7 +353,7 @@ int mjb_step_profile(const mjbModel* m, mjbData* d, void* stream, float* ms_out)
   while (n < 7 && !(rc = check(cudaEventCreate(&ev[n]), "cudaEventCreate"))) n++;
   if (!rc) rc = check(reset_contact_counters(d->dev, s), "reset_contact_counters");
   if (!rc) rc = check(cudaEventRecord(ev[0], s), "cudaEventRecord");
-  if (!rc) rc = chain(m, d->dev, RUN_POSITION | RUN_VELOCITY | RUN_SOLVER | RUN_EULER, s, ev + 1);
+  if (!rc) rc = chain(m, d, d->dev, RUN_POSITION | RUN_VELOCITY | RUN_SOLVER | RUN_EULER, s, ev + 1);
   if (!rc) rc = check(cudaEventSynchronize(ev[6]), "cudaEventSynchronize");
   for (int i = 0; i < 6 && !rc; i++) rc = check(cudaEventElapsedTime(&ms_out[i], ev[i], ev[i + 1]), "cudaEventElapsedTime");
   for (int i = 0; i < n; i++) cudaEventDestroy(ev[i]);

@@ -153,30 +153,7 @@ __device__ __forceinline__ int update_constraint(Ctx& c, bool init) {
       const float jaref = c.Jaref[r], D = c.D[r];
       const int old = c.state[r];
       float force; int st;
-      if (r < c.ne) { force = -D * jaref; st = ST_QUADRATIC; }
-      else if (r < c.ne + c.nf) {
-        const float f = c.floss[r], rf = safe_div(f, D);
-        if (jaref <= -rf) { force = f; st = ST_LINEARNEG; } else if (jaref >= rf) { force = -f; st = ST_LINEARPOS; } else { force = -D * jaref; st = ST_QUADRATIC; }
-      } else if (ELL && c.rinfo[r] != -1) {  // solver.py:455-472
-        const int info = c.rinfo[r];
-        force = 0.f; st = ST_SATISFIED;
-        if (info >= 0) {
-          const int j = info & 15, dim = info >> 4, e0 = r - j;
-          const float mu = c.rfri[e0], N = c.Jaref[e0] * mu;
-          float TT = 0.f;
-          for (int i = 1; i < dim; i++) { const float u = c.Jaref[e0 + i] * c.rfri[e0 + i]; TT += u * u; }
-          const float T = TT <= 0.f ? 0.f : sqrtf(TT);
-          if ((N >= mu * T) || (T <= 0.f && N >= 0.f)) {}
-          else if ((mu * N + T <= 0.f) || (T <= 0.f && N < 0.f)) { force = -D * jaref; st = ST_QUADRATIC; }
-          else {
-            const float dm = safe_div(c.D[e0], mu * mu * (1.0f + mu * mu)), fn = -dm * (N - mu * T) * mu, fr = c.rfri[r];
-            force = j == 0 ? fn : -safe_div(fn, T) * (jaref * fr * fr);
-            st = ST_CONE;
-            cone0 = j == 0;
-          }
-        }
-      } else if (jaref >= 0.f) { force = 0.f; st = ST_SATISFIED; }
-      else { force = -D * jaref; st = ST_QUADRATIC; }
+      MJB_ROW_FORCE_STATE(ELL, r, c.ne, c.nf, jaref, D, c.floss, c.rinfo, c.rfri, c.Jaref, c.D, force, st, cone0)
       c.force[r] = force; c.state[r] = st;
       const bool nq = st == ST_QUADRATIC, oq = (!init) && old == ST_QUADRATIC;
       flip = nq != oq;

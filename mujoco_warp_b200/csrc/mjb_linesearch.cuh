@@ -55,6 +55,44 @@ __device__ __forceinline__ P3 eval_gauss(float q0, float q1, float q2, float alp
 }
 __device__ __forceinline__ bool in_bracket(P3 x, P3 y) { return (x.g < y.g && y.g < 0.f) || (x.g > y.g && y.g > 0.f); }
 
+// ---- force and state of one row at its Jaref (solver.py:1699 _update_constraint_efc), shared by the solver's row pass (k_solver.cu) and
+// inverse dynamics (k_inverse.cu).  Row kinds by position as above; with ELL, rows whose rinfo is not -1 belong to an elliptic contact:
+// rinfo = -2 (contact cut by njmax: no force) or (dim << 4) | j, and rfri = mu (j = 0) or friction[j - 1].  Jaref, Dv: the world's rows.
+// Sets force and st, and cone0 = true when the row is the first row of a contact in the cone zone.  A macro, so that the solver's row pass
+// compiles exactly as it did with the rule written out in place (the inlined-function form reorders its branches).
+#define MJB_ROW_FORCE_STATE(ELL, r, ne, nf, jaref, D, floss, rinfo, rfri, Jaref, Dv, force, st, cone0)                                          \
+  if ((r) < (ne)) { force = -(D) * (jaref); st = ST_QUADRATIC; }                                                                            \
+  else if ((r) < (ne) + (nf)) {                                                                                                              \
+    const float f_ = (floss)[r], rf_ = safe_div(f_, D);                                                                                      \
+    if ((jaref) <= -rf_) { force = f_; st = ST_LINEARNEG; } else if ((jaref) >= rf_) { force = -f_; st = ST_LINEARPOS; }                      \
+    else { force = -(D) * (jaref); st = ST_QUADRATIC; }                                                                                      \
+  } else if ((ELL) && (rinfo)[r] != -1) {  /* solver.py:455-472 */                                                                           \
+    const int info_ = (rinfo)[r];                                                                                                            \
+    force = 0.f; st = ST_SATISFIED;                                                                                                          \
+    if (info_ >= 0) {                                                                                                                        \
+      const int j_ = info_ & 15, dim_ = info_ >> 4, e0_ = (r) - j_;                                                                          \
+      const float mu_ = (rfri)[e0_], N_ = (Jaref)[e0_] * mu_;                                                                                \
+      float TT_ = 0.f;                                                                                                                       \
+      for (int i_ = 1; i_ < dim_; i_++) { const float u_ = (Jaref)[e0_ + i_] * (rfri)[e0_ + i_]; TT_ += u_ * u_; }                          \
+      const float T_ = TT_ <= 0.f ? 0.f : sqrtf(TT_);                                                                                        \
+      if ((N_ >= mu_ * T_) || (T_ <= 0.f && N_ >= 0.f)) {}                                                                                   \
+      else if ((mu_ * N_ + T_ <= 0.f) || (T_ <= 0.f && N_ < 0.f)) { force = -(D) * (jaref); st = ST_QUADRATIC; }                             \
+      else {                                                                                                                                 \
+        const float dm_ = safe_div((Dv)[e0_], mu_ * mu_ * (1.0f + mu_ * mu_)), fn_ = -dm_ * (N_ - mu_ * T_) * mu_, fr_ = (rfri)[r];          \
+        force = j_ == 0 ? fn_ : -safe_div(fn_, T_) * ((jaref) * fr_ * fr_);                                                                   \
+        st = ST_CONE;                                                                                                                        \
+        cone0 = j_ == 0;                                                                                                                     \
+      }                                                                                                                                      \
+    }                                                                                                                                        \
+  } else if ((jaref) >= 0.f) { force = 0.f; st = ST_SATISFIED; }                                                                             \
+  else { force = -(D) * (jaref); st = ST_QUADRATIC; }
+
+template <bool ELL>
+__device__ __forceinline__ void row_force_state(int r, int ne, int nf, float jaref, float D, const float* floss, const int* rinfo, const float* rfri,
+                                                const float* Jaref, const float* Dv, float& force, int& st, bool& cone0) {
+  MJB_ROW_FORCE_STATE(ELL, r, ne, nf, jaref, D, floss, rinfo, rfri, Jaref, Dv, force, st, cone0)
+}
+
 // ---- elliptic cone, one contact (quad = cost polynomial of all its rows, (u0, v0, uu), (uv, vv, dm))
 struct EllQ { float q0, q1, q2, u0, v0, uu, uv, vv, dm; };
 struct EllRef { float cost0, T0, r0; int st; };

@@ -135,6 +135,7 @@ enum {
   DSBL_SPRING = 1 << 5, DSBL_DAMPER = 1 << 6, DSBL_GRAVITY = 1 << 7, DSBL_CLAMPCTRL = 1 << 8, DSBL_WARMSTART = 1 << 9,
   DSBL_ACTUATION = 1 << 11, DSBL_REFSAFE = 1 << 12, DSBL_SENSOR = 1 << 13, DSBL_EULERDAMP = 1 << 15, DSBL_NATIVECCD = 1 << 17
 };
+enum { ENBL_INVDISCRETE = 1 << 3 };
 enum { OVF_NEFC = 1 << 0, OVF_NJMAX_NNZ = 1 << 1, OVF_BROADPHASE = 1 << 2, OVF_NARROWPHASE = 1 << 3, OVF_EPA_HORIZON = 1 << 8, OVF_ITERATIONS = 1 << 9, OVF_LS_ITERATIONS = 1 << 10 };
 enum { BF_PLANE = 1, BF_SPHERE = 2, BF_AABB = 4, BF_OBB = 8 };
 enum { CONTACT_TYPE_CONSTRAINT = 1, CONTACT_TYPE_SENSOR = 2 };
@@ -168,6 +169,9 @@ cudaError_t launch_implicit_solve(const ModelDev& m, const DataDev& d, float* qa
 size_t smem_implicit(const ModelDev& m);
 cudaError_t launch_sensor(const ModelDev& m, const DataDev& d, int stages, cudaStream_t s);
 cudaError_t launch_contact_force(const ModelDev& m, const DataDev& d, const int* contact_ids, int n, int to_world, float* out, cudaStream_t s);
+// inverse dynamics at the given d.qacc into qfrc_inverse (nworld, nv); disc: d.qacc is a discrete-time acceleration, converted first,
+// and the continuous one goes to qacc_cont (nworld, nv) (k_inverse.cu)
+cudaError_t launch_inverse(const ModelDev& m, const DataDev& d, float* qfrc_inverse, float* qacc_cont, bool disc, cudaStream_t s);
 cudaError_t launch_rk_stage(const ModelDev& m, const DataDev& d, float* rk, int stage, cudaStream_t s);
 // rays (nworld x nray, world-major) against every geom of every world; geomgroup: 6 ints, all -1 = no group filter (k_ray.cu)
 cudaError_t launch_ray(const ModelDev& m, const DataDev& d, const float* pnt, const float* vec, int nray, int pnt_nbatch, const int* geomgroup, int flg_static,
