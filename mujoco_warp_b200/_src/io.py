@@ -281,6 +281,11 @@ def derive_tables(mjm) -> dict:
   return t
 
 
+def _has_fluid(o) -> bool:
+  """io.py:471: the model has fluid forces."""
+  return bool(np.any(np.asarray(getattr(o, "wind", 0.0)) != 0.0) or float(getattr(o, "density", 0.0)) > 0.0 or float(getattr(o, "viscosity", 0.0)) > 0.0)
+
+
 def _validate(mjm):
   """Feature checks in the spirit of io.py:284-363: fail loudly on anything the kernels do not cover."""
   o = mjm.opt
@@ -293,8 +298,8 @@ def _validate(mjm):
   if o.solver not in (C.SOL_NEWTON, C.SOL_CG):
     raise NotImplementedError("only the Newton and CG solvers are implemented in this version (no PGS)")
   # features the kernels do not evaluate must fail here, not silently change the simulation (ADVICE r1)
-  if float(getattr(o, "density", 0.0)) != 0.0 or float(getattr(o, "viscosity", 0.0)) != 0.0 or np.any(np.asarray(getattr(o, "wind", 0.0)) != 0.0):
-    raise NotImplementedError("fluid forces (opt.density / viscosity / wind) are not implemented")
+  if _has_fluid(o) and o.integrator == C.INT_IMPLICIT:
+    raise NotImplementedError("fluid forces (opt.density / viscosity / wind) with the implicit integrator are not implemented (use implicitfast, Euler or RK4)")
   if int(getattr(o, "noslip_iterations", 0)) > 0:
     raise NotImplementedError("the noslip solver (opt.noslip_iterations > 0) is not implemented")
   unsupported_enable = int(o.enableflags) & (C.ENBL_OVERRIDE | C.ENBL_ENERGY | C.ENBL_FWDINV | C.ENBL_SLEEP)
@@ -387,6 +392,9 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
     disableflags=int(o.disableflags), enableflags=int(o.enableflags), impratio_invsqrt=f32(1.0 / np.sqrt(o.impratio)),
     broadphase=types.BroadphaseType(int(getattr(o, "broadphase", 0))), broadphase_filter=int(getattr(o, "broadphase_filter", C.BF_PLANE | C.BF_SPHERE | C.BF_OBB)),
     graph_conditional=False, run_collision_detection=True, warn_overflow=False,
+    # model constants here, one value for every world (the reference indexes them per world)
+    density=f32(float(getattr(o, "density", 0.0))), viscosity=f32(float(getattr(o, "viscosity", 0.0))),
+    wind=f32(np.asarray(getattr(o, "wind", np.zeros(3)), dtype=np.float64).reshape(3)),
   )
   if len(t["nxn_geom_pair_filtered"]) >= 250_000:
     # the reference switches to sweep-and-prune here (io.py:631-636); this build keeps one world's geoms and pair list in one
@@ -511,6 +519,20 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   m.mesh_faceadr = dev_i(getattr(mjm, "mesh_faceadr", np.zeros(nmesh)) if nmesh else np.zeros(0))
   m.mesh_face = dev_i(np.asarray(getattr(mjm, "mesh_face", np.zeros((0, 3)))).reshape(-1, 3) if nmesh else np.zeros((0, 3)))
   m.nmeshface = int(m.mesh_face.shape[0])
+  # fluid forces (io.py:471, 523-530).  Models saved without geom_fluid have no ellipsoid geoms.
+  m.has_fluid = _has_fluid(o)
+  geom_fluid = np.asarray(getattr(mjm, "geom_fluid", np.zeros((ng, 12))), dtype=np.float64).reshape(ng, 12)
+  m.geom_fluid = dev_f(geom_fluid, batched=False)
+  ellipsoid = np.zeros(m.nbody, dtype=bool)
+  ellipsoid[np.asarray(mjm.geom_bodyid)[geom_fluid[:, 0] > 0]] = True
+  box = ~ellipsoid & (np.asarray(mjm.body_mass) > 0.0)
+  box[0] = False
+  m.body_fluid_ellipsoid = torch.from_numpy(ellipsoid).to(dev)
+  m.body_fluid_ellipsoid_adr = dev_i(np.nonzero(ellipsoid)[0])
+  m.body_fluid_box_adr = dev_i(np.nonzero(box)[0])
+  m.body_fluid = dev_i(np.where(ellipsoid, 1, np.where(box, 2, 0)))  # the kernels' per-body model: 0 none, 1 ellipsoid, 2 inertia box
+  m.body_geomadr = dev_i(mjm.body_geomadr)
+  m.body_geomnum = dev_i(mjm.body_geomnum)
   m.M_mulm_rowadr, m.M_mulm_col, m.M_mulm_madr = m.mulm_rowadr, m.mulm_col, m.mulm_madr
   anc_pad = np.zeros((m.nbody, m.nv_pad), dtype=np.int32)
   anc_pad[:, : m.nv] = t["body_isdofancestor"]
@@ -530,13 +552,15 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
     iterations=m.opt.iterations, ls_iterations=m.opt.ls_iterations, disableflags=m.opt.disableflags, enableflags=m.opt.enableflags,
     broadphase=int(m.opt.broadphase), broadphase_filter=m.opt.broadphase_filter, qld_total=t["qld_total"], maxtree=t["maxtree"],
     has_multicontact_geom=int(np.isin(_np(mjm, "geom_type"), (C.GEOM_ELLIPSOID, C.GEOM_CYLINDER, C.GEOM_BOX, C.GEOM_MESH)).any()), nmesh=nmesh, na=m.na, ntendon=m.ntendon, nJten=m.nJten, ntenfric=m.ntenfric, nwrap=m.nwrap,
-    nmocap=int(getattr(mjm, "nmocap", 0)), npair=npair, has_convex_pair=t["has_convex_pair"], ccd_iterations=int(getattr(o, "ccd_iterations", 35)), epa_iterations=t["epa_iterations"], nsensor=m.nsensor, nsensordata=m.nsensordata, nmat=m.nmat, nmeshface=m.nmeshface, sensor_subtree_vel=int(m.sensor_subtree_vel), sensor_rne_postconstraint=int(m.sensor_rne_postconstraint), neq=neq, nlimit_ball=len(t["jnt_limited_ball_adr"]), has_gravcomp=int((np.asarray(mjm.body_gravcomp) != 0).any() or (np.asarray(mjm.jnt_stiffness)[np.isin(np.asarray(mjm.jnt_type), (C.JNT_FREE, C.JNT_BALL))] != 0).any()),
+    nmocap=int(getattr(mjm, "nmocap", 0)), npair=npair, has_convex_pair=t["has_convex_pair"], ccd_iterations=int(getattr(o, "ccd_iterations", 35)), epa_iterations=t["epa_iterations"], nsensor=m.nsensor, nsensordata=m.nsensordata, nmat=m.nmat, nmeshface=m.nmeshface, sensor_subtree_vel=int(m.sensor_subtree_vel), sensor_rne_postconstraint=int(m.sensor_rne_postconstraint), neq=neq, nlimit_ball=len(t["jnt_limited_ball_adr"]), has_fluid=int(m.has_fluid), has_gravcomp=int((np.asarray(mjm.body_gravcomp) != 0).any() or (np.asarray(mjm.jnt_stiffness)[np.isin(np.asarray(mjm.jnt_type), (C.JNT_FREE, C.JNT_BALL))] != 0).any()),
   )
   for k, v in ints.items():
     _lib.check(L.mjb_model_set_int(h, k.encode(), int(v)))
   g = np.asarray(o.gravity, dtype=np.float64)
   floats = dict(timestep=o.timestep, tolerance=tol, ls_tolerance=o.ls_tolerance, impratio_invsqrt=1.0 / np.sqrt(o.impratio),
                 meaninertia=mjm.stat.meaninertia, gravity_x=g[0], gravity_y=g[1], gravity_z=g[2], ccd_tolerance=float(getattr(o, "ccd_tolerance", 1e-6)))
+  wind = np.asarray(getattr(o, "wind", np.zeros(3)), dtype=np.float64).reshape(3)
+  floats.update(density=float(getattr(o, "density", 0.0)), viscosity=float(getattr(o, "viscosity", 0.0)), wind_x=wind[0], wind_y=wind[1], wind_z=wind[2])
   for k, v in floats.items():
     _lib.check(L.mjb_model_set_float(h, k.encode(), float(v)))
   dev_names = {
@@ -553,7 +577,8 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
                                          "mesh_polymap", "mesh_vert", "mesh_polynormal", "actuator_dyntype", "actuator_actadr", "actuator_actnum",
                                          "actuator_actlimited", "actuator_actearly", "actuator_dynprm", "actuator_actrange", "actuator_trntype",
                                          "ten_J_rownnz", "ten_J_rowadr", "ten_J_colind", "tendon_adr", "tendon_num", "wrap_objid", "tendon_limited", "tendon_actfrclimited", "wrap_prm", "ten_J0",
-                                         "geom_group", "geom_matid", "geom_rgba", "mat_rgba", "mesh_faceadr", "mesh_face"]
+                                         "geom_group", "geom_matid", "geom_rgba", "mat_rgba", "mesh_faceadr", "mesh_face",
+                                         "geom_fluid", "body_fluid", "body_geomadr", "body_geomnum"]
                                         + [n for n, _ in _TENDON_FLOATS]):
     dev_names.setdefault(n, getattr(m, n))
   for n, x in dev_names.items():
@@ -568,7 +593,8 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   return m
 
 
-_OPT_FLOATS = {"timestep": "timestep", "tolerance": "tolerance", "ls_tolerance": "ls_tolerance", "impratio_invsqrt": "impratio_invsqrt", "ccd_tolerance": "ccd_tolerance"}
+_OPT_FLOATS = {"timestep": "timestep", "tolerance": "tolerance", "ls_tolerance": "ls_tolerance", "impratio_invsqrt": "impratio_invsqrt", "ccd_tolerance": "ccd_tolerance",
+               "density": "density", "viscosity": "viscosity"}
 _OPT_INTS = ("integrator", "cone", "solver", "iterations", "ls_iterations", "disableflags", "enableflags", "broadphase", "broadphase_filter", "ccd_iterations")
 
 
@@ -610,11 +636,11 @@ def _install_model_rebind(m: types.Model, L, arrays, ints):
         v = max(v, 1e-6)
       _lib.check(L.mjb_model_set_float(h, _OPT_FLOATS[name].encode(), v))
       return torch.full((1,), v, dtype=torch.float32, device=m.opt.__dict__[name].device) if not isinstance(value, torch.Tensor) else value
-    if name == "gravity":
+    if name in ("gravity", "wind"):
       g = value.reshape(-1)[:3].tolist() if isinstance(value, torch.Tensor) else [float(x) for x in value]
-      for k, v in zip(("gravity_x", "gravity_y", "gravity_z"), g):
+      for k, v in zip((f"{name}_x", f"{name}_y", f"{name}_z"), g):
         _lib.check(L.mjb_model_set_float(h, k.encode(), float(v)))
-      return value if isinstance(value, torch.Tensor) else torch.tensor([g], dtype=torch.float32, device=m.opt.__dict__["gravity"].device)
+      return value if isinstance(value, torch.Tensor) else torch.tensor([g], dtype=torch.float32, device=m.opt.__dict__[name].device)
     if name in _OPT_INTS:
       if name == "integrator" and int(value) not in (C.INT_EULER, C.INT_IMPLICIT, C.INT_IMPLICITFAST, C.INT_RK4):
         raise NotImplementedError(f"integrator {value} not implemented")
@@ -697,7 +723,7 @@ _BOUND_TOP = [
   "crb", "M", "qLD", "actuator_length", "actuator_moment", "actuator_velocity", "cvel", "cdof_dot", "qfrc_bias", "qfrc_spring", "qfrc_damper",
   "qfrc_gravcomp", "qfrc_passive", "actuator_force", "qfrc_actuator", "qfrc_smooth", "qacc_smooth", "qfrc_constraint", "qfrc_inverse", "cacc", "cfrc_int",
   "ne", "nf", "nl", "nefc", "nacon", "ncollision", "solver_niter", "overflow", "moment_rownnz", "moment_rowadr", "moment_colind", "eq_active", "mocap_pos", "mocap_quat", "sensordata", "subtree_linvel", "subtree_angmom", "cfrc_ext",
-  "act", "act_dot", "ten_length", "ten_J", "ten_velocity", "qLU",
+  "act", "act_dot", "ten_length", "ten_J", "ten_velocity", "qLU", "qfrc_fluid",
 ]
 _BOUND_EFC = ["J", "pos", "margin", "D", "vel", "aref", "frictionloss", "force", "Ma", "type", "id", "state"]
 _BOUND_CONTACT = ["dist", "pos", "frame", "includemargin", "friction", "solref", "solreffriction", "solimp", "dim", "geom", "efc_address", "worldid", "type", "geomcollisionid"]

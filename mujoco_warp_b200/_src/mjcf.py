@@ -193,6 +193,67 @@ def _geom_volume_inertia(gtype, size):
   return 0.0, np.zeros(3)
 
 
+def fluid_semiaxes(gtype, size):
+  """Semi-axes of the ellipsoid the fluid model puts in place of a geom (reference passive.py:46 geom_semiaxes)."""
+  if gtype == C.GEOM_SPHERE:
+    return np.array([size[0], size[0], size[0]], dtype=np.float64)
+  if gtype == C.GEOM_CAPSULE:
+    return np.array([size[0], size[0], size[1] + size[0]], dtype=np.float64)
+  if gtype == C.GEOM_CYLINDER:
+    return np.array([size[0], size[0], size[1]], dtype=np.float64)
+  return np.asarray(size, dtype=np.float64)[:3].copy()
+
+
+def _carlson_rd(x, y, z):
+  """Carlson's symmetric elliptic integral R_D(x, y, z) = 3/2 int_0^inf dt / ((t + z) sqrt((t + x)(t + y)(t + z))), by duplication."""
+  s, fac = 0.0, 1.0
+  for _ in range(100):
+    mu = (x + y + 3.0 * z) / 5.0
+    ex, ey, ez = (mu - x) / mu, (mu - y) / mu, (mu - z) / mu
+    if max(abs(ex), abs(ey), abs(ez)) < 1e-4:
+      break
+    sx, sy, sz = math.sqrt(x), math.sqrt(y), math.sqrt(z)
+    lam = sx * (sy + sz) + sy * sz
+    s += fac / (sz * (z + lam))
+    fac *= 0.25
+    x, y, z = 0.25 * (x + lam), 0.25 * (y + lam), 0.25 * (z + lam)
+  ea, eb = ex * ey, ez * ez
+  ec, ed = ea - eb, ea - 6.0 * eb
+  ee = ed + ec + ec
+  series = 1.0 + ed * (-3.0 / 14.0 + 9.0 / 88.0 * ed - 4.5 / 26.0 * ez * ee) + ez * (ee / 6.0 + ez * (-9.0 / 22.0 * ec + ez * 3.0 / 26.0 * ea))
+  return 3.0 * s + fac * series / (mu * math.sqrt(mu))
+
+
+def fluid_kappa(s):
+  """Lamb's added-mass integrals kappa_i = a b c int_0^inf dl / ((a_i^2 + l) sqrt((a^2 + l)(b^2 + l)(c^2 + l))) of an ellipsoid with
+  semi-axes s = (a, b, c).  They sum to 2; a sphere has 2/3 on every axis."""
+  a2 = [float(v) * float(v) for v in s]
+  abc = float(s[0]) * float(s[1]) * float(s[2])
+  return np.array([abc * 2.0 / 3.0 * _carlson_rd(a2[(i + 1) % 3], a2[(i + 2) % 3], a2[i]) for i in range(3)])
+
+
+def geom_fluid_row(gtype, size, fluidshape, fluidcoef):
+  """One row of Model.geom_fluid (12 numbers, MuJoCo's layout): [0] the ellipsoid-model flag, [1:6] blunt drag, slender drag, angular
+  drag, Kutta lift and Magnus lift coefficients, [6:9] virtual mass and [9:12] virtual inertia of the geom's fluid ellipsoid per unit
+  fluid density.  A geom with fluidshape="none" gets a row of zeros."""
+  row = np.zeros(12)
+  if fluidshape != "ellipsoid":
+    return row
+  s = fluid_semiaxes(gtype, size)
+  k = fluid_kappa(s)
+  vol = 4.0 / 3.0 * math.pi * s[0] * s[1] * s[2]
+  row[0] = 1.0
+  row[1:6] = fluidcoef
+  row[6:9] = vol * k / np.maximum(C.MJ_MINVAL, 2.0 - k)
+  sq = s * s
+  for i in range(3):  # Lamb's added moment of inertia about axis i, from the two other axes j, k
+    j, l = (i + 1) % 3, (i + 2) % 3
+    num = (sq[j] - sq[l]) ** 2 * abs(k[l] - k[j])
+    den = max(C.MJ_MINVAL, abs(2.0 * (sq[j] - sq[l]) + (sq[j] + sq[l]) * (k[j] - k[l])))
+    row[9 + i] = vol * num / den / 5.0
+  return row
+
+
 def _geom_rbound(gtype, size):
   if gtype == C.GEOM_SPHERE:
     return size[0]
@@ -778,7 +839,10 @@ def compile_xml(root):
           rgba=_vec(a.get("rgba"), 4, default=[0.5, 0.5, 0.5, 1.0]),
           matid=mat_names.index(a["material"]) if a.get("material") in mat_names else -1,
           dataid=dataid,
+          fluid=geom_fluid_row(gtype, size, a.get("fluidshape", "none"), _vec(a.get("fluidcoef"), 5, default=C.DEFAULT_FLUIDCOEF)),
         )
+        if a.get("fluidshape", "none") not in ("none", "ellipsoid"):
+          raise ValueError(f"geom fluidshape must be 'none' or 'ellipsoid', got {a['fluidshape']!r}")
         if b["geomnum"] == 0:
           b["geomadr"] = len(geoms)
         b["geomnum"] += 1
@@ -993,6 +1057,7 @@ def compile_xml(root):
   m.geom_group = np.array([g["group"] for g in geoms], dtype=np.int32).reshape(ngeom)
   m.geom_matid = np.array([g["matid"] for g in geoms], dtype=np.int32).reshape(ngeom)
   m.geom_rgba = np.array([g["rgba"] for g in geoms]).reshape(ngeom, 4)
+  m.geom_fluid = np.array([g["fluid"] for g in geoms]).reshape(ngeom, 12)
   m.nmat = len(mat_names)
   m.mat_rgba = np.array(mat_rgba).reshape(m.nmat, 4)
   m.names.material = list(mat_names)

@@ -12,6 +12,7 @@ using std::min;
 
 struct mjbModel {
   ModelDev dev;
+  FluidDev fluid;  // qfrc_fluid stays null here: it is the Data's (fluid() below)
   bool finalized;
 };
 struct mjbData {
@@ -26,6 +27,7 @@ struct mjbData {
   // inverse dynamics (k_inverse.cu takes them as arguments: DataDev stays as the other kernels know it)
   float* qfrc_inverse;  // Data.qfrc_inverse, (nworld, nv), bound by name like the DataDev arrays
   float* inv_qacc;      // (nworld, nv) continuous-time acceleration of discrete inverse dynamics, read by its sensor launch
+  float* qfrc_fluid;    // Data.qfrc_fluid, (nworld, nv), bound by name; passed to the fluid kernels in FluidDev
 };
 
 namespace {
@@ -38,6 +40,9 @@ int check(cudaError_t e, const char* what) {
 constexpr size_t kMaxSmem = 227 * 1024;
 }  // namespace
 
+// The fluid fields of a model bound to a Data's qfrc_fluid
+static FluidDev fluid(const mjbModel* m, const mjbData* d) { FluidDev f = m->fluid; f.qfrc_fluid = d->qfrc_fluid; return f; }
+
 extern "C" {
 
 const char* mjb_last_error(void) { return g_err.c_str(); }
@@ -47,6 +52,7 @@ int mjb_last_launch_count(void) { return g_launches; }
 mjbModel* mjb_model_create(void) {
   mjbModel* m = new mjbModel();
   memset(&m->dev, 0, sizeof(ModelDev));
+  memset(&m->fluid, 0, sizeof(FluidDev));
   m->finalized = false;
   return m;
 }
@@ -56,11 +62,17 @@ int mjb_model_set_int(mjbModel* m, const char* name, int v) {
 #define X(n) if (!strcmp(name, #n)) { m->dev.n = v; return 0; }
   MJB_MODEL_INTS(X)
 #undef X
+#define X(n) if (!strcmp(name, #n)) { m->fluid.n = v; return 0; }
+  MJB_FLUID_INTS(X)
+#undef X
   return fail(std::string("unknown model int field: ") + name);
 }
 int mjb_model_set_float(mjbModel* m, const char* name, float v) {
 #define X(n) if (!strcmp(name, #n)) { m->dev.n = v; return 0; }
   MJB_MODEL_FLOATS(X)
+#undef X
+#define X(n) if (!strcmp(name, #n)) { m->fluid.n = v; return 0; }
+  MJB_FLUID_FLOATS(X)
 #undef X
   return fail(std::string("unknown model float field: ") + name);
 }
@@ -68,6 +80,10 @@ int mjb_model_set_array_batched(mjbModel* m, const char* name, const void* p, in
   if (nbatch < 1) return fail(std::string("nbatch must be >= 1: ") + name);
 #define X(n) if (!strcmp(name, #n)) { if (nbatch != 1) return fail(std::string("integer Model tables are shared by all worlds (not batched): ") + name); m->dev.n = (const int*)p; return 0; }
   MJB_MODEL_IARRS(X)
+#undef X
+#define X(n) if (!strcmp(name, #n)) { if (nbatch != 1) return fail(std::string("shared by all worlds (not batched): ") + name); m->fluid.n = (decltype(m->fluid.n))p; return 0; }
+  MJB_FLUID_IARRS(X)
+  MJB_FLUID_FARRS(X)
 #undef X
 #define X(n) if (!strcmp(name, #n)) { m->dev.n = (const float*)p; m->dev.nb_##n = nbatch; m->dev.bs_##n = batch_stride; goto done; }
   MJB_MODEL_FARRS(X)
@@ -89,6 +105,10 @@ int mjb_model_finalize(mjbModel* m) {
   MJB_MODEL_IARRS(X)
   MJB_MODEL_FARRS(X)
 #undef X
+#define X(n) if (!m->fluid.n) return fail(std::string("model array not set: ") + #n);
+  MJB_FLUID_IARRS(X)
+  MJB_FLUID_FARRS(X)
+#undef X
   if (m->dev.nv <= 0 || m->dev.nbody <= 0) return fail("model has no dofs/bodies");
   if (m->dev.solver != SOL_NEWTON && m->dev.solver != SOL_CG) return fail("only the Newton and CG solvers are implemented");
   if (m->dev.cone != CONE_PYRAMIDAL && m->dev.cone != CONE_ELLIPTIC) return fail("unknown friction cone type");
@@ -108,6 +128,7 @@ mjbData* mjb_data_create(int nworld, int nconmax, int naconmax, int njmax, int n
   d->rk = nullptr;
   d->qfrc_inverse = nullptr;
   d->inv_qacc = nullptr;
+  d->qfrc_fluid = nullptr;
   return d;
 }
 void mjb_data_destroy(mjbData* d) {
@@ -129,6 +150,7 @@ int mjb_data_set_int(mjbData* d, const char* name, int v) {
 }
 int mjb_data_set_array(mjbData* d, const char* name, void* p) {
   if (!strcmp(name, "qfrc_inverse")) { d->qfrc_inverse = (float*)p; return 0; }
+  if (!strcmp(name, "qfrc_fluid")) { d->qfrc_fluid = (float*)p; return 0; }
 #define X(n) if (!strcmp(name, #n)) { d->dev.n = (float*)p; return 0; }
   MJB_DATA_FARRS(X)
 #undef X
@@ -144,6 +166,7 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
   MJB_DATA_IARRS(X)
 #undef X
   if (!d->qfrc_inverse) return fail("data array not set: qfrc_inverse");
+  if (!d->qfrc_fluid) return fail("data array not set: qfrc_fluid");
   if (d->dev.nv_pad < m->dev.nv) return fail("nv_pad < nv");
   if (check(cudaMalloc(&d->dev.world_conadr, sizeof(int) * (size_t)d->dev.nworld), "cudaMalloc(world_conadr)")) return -1;
   if (check(cudaMalloc(&d->dev.world_ncon, sizeof(int) * (size_t)d->dev.nworld), "cudaMalloc(world_ncon)")) return -1;
@@ -156,7 +179,7 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
   if (m->dev.integrator == INT_RK4 && !d->rk &&
       check(cudaMalloc(&d->rk, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nq + 3 * m->dev.nv + 2 * m->dev.na + 1)), "cudaMalloc(rk)")) return -1;
   const size_t smem[6] = {smem_position(m->dev, d->dev), smem_collision(m->dev, d->dev), smem_constraint(m->dev, d->dev),
-                          smem_velocity(m->dev, d->dev), smem_solver(m->dev, d->dev),    smem_integrate(m->dev)};
+                          smem_velocity(m->dev, d->dev, fluid(m, d)), smem_solver(m->dev, d->dev),    smem_integrate(m->dev)};
   static const char* names[6] = {"position", "collision", "constraint", "velocity", "solver", "integrate"};
   for (int i = 0; i < 6; i++)
     if (smem[i] > kMaxSmem) {
@@ -199,13 +222,13 @@ int mjb_make_constraint(const mjbModel* m, mjbData* d, void* stream) {
   if (d->dev.njmax_nnz > 0) MJB_LAUNCH(launch_efc_csr(m->dev, d->dev, s));
   return 0;
 }
-int mjb_fwd_velocity(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_VELOCITY, s)); return 0; }
-int mjb_fwd_actuation(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_ACTUATION, s)); return 0; }
-int mjb_fwd_acceleration(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_ACCELERATION, s)); return 0; }
-int mjb_factor_m(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_FACTOR_ONLY, s)); return 0; }
-int mjb_com_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_COMVEL, s)); return 0; }
-int mjb_passive(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_PASSIVE, s)); return 0; }
-int mjb_rne(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_RNE, s)); return 0; }
+int mjb_fwd_velocity(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_VELOCITY, s, fluid(m, d))); return 0; }
+int mjb_fwd_actuation(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_ACTUATION, s, fluid(m, d))); return 0; }
+int mjb_fwd_acceleration(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_ACCELERATION, s, fluid(m, d))); return 0; }
+int mjb_factor_m(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_FACTOR_ONLY, s, fluid(m, d))); return 0; }
+int mjb_com_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_COMVEL, s, fluid(m, d))); return 0; }
+int mjb_passive(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_PASSIVE, s, fluid(m, d))); return 0; }
+int mjb_rne(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_RNE, s, fluid(m, d))); return 0; }
 int mjb_solve_m(const mjbModel* m, mjbData* d, float* x, const float* y, void* stream) {
   MJB_ENTER();
   if (!x || !y) return fail("mjb_solve_m: null vector");
@@ -239,7 +262,7 @@ int mjb_sensor_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); M
 int mjb_sensor_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 2, s)); return 0; }
 int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 4, s)); return 0; }
 int mjb_solve(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_solver(m->dev, d->dev, s)); return 0; }
-int mjb_euler(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_integrate(m->dev, d->dev, INT_EULER, s)); return 0; }
+int mjb_euler(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_integrate(m->dev, d->dev, INT_EULER, s, fluid(m, d))); return 0; }
 
 // which stages a pipeline call runs
 enum { RUN_POSITION = 1, RUN_VELOCITY = 2, RUN_SOLVER = 4, RUN_EULER = 8, RUN_INVERSE = 16 };
@@ -266,7 +289,7 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
     MJB_MARK(2);
   }
   if (what & RUN_VELOCITY) {
-    MJB_LAUNCH(launch_velocity(m->dev, dd, STG_VELOCITY | STG_ACTUATION | STG_ACCELERATION, s));
+    MJB_LAUNCH(launch_velocity(m->dev, dd, STG_VELOCITY | STG_ACTUATION | STG_ACCELERATION, s, fluid(m, d)));
     MJB_MARK(3);
   }
   if (what & RUN_SOLVER) {
@@ -279,7 +302,7 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
     // inverse dynamics at the given qacc, then the sensors of all three stages; with a discrete-time qacc they read the continuous
     // one k_inverse wrote to the scratch, and d.qacc itself is never written
     const bool disc = inverse_discrete(m->dev);
-    MJB_LAUNCH(launch_inverse(m->dev, dd, d->qfrc_inverse, d->inv_qacc, disc, s));
+    MJB_LAUNCH(launch_inverse(m->dev, dd, d->qfrc_inverse, d->inv_qacc, disc, s, fluid(m, d)));
     if (m->dev.nsensor > 0) {
       DataDev ds = dd;
       if (disc) ds.qacc = d->inv_qacc;
@@ -288,7 +311,7 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
   }
   if (what & RUN_EULER) {
     if (m->dev.integrator == INT_IMPLICIT && smem_implicit(m->dev) > kMaxSmem) return fail("implicit integrator: the velocity-derivative scratch (18 x nbody x 32 floats) exceeds one block's shared memory");
-    MJB_LAUNCH(launch_integrate(m->dev, dd, -1, s));
+    MJB_LAUNCH(launch_integrate(m->dev, dd, -1, s, fluid(m, d)));
     MJB_MARK(5);
   }
 #undef MJB_MARK
@@ -363,7 +386,7 @@ int mjb_team_residency(const mjbModel* m, const mjbData* d, int* position_worlds
   if (!m || !d || !m->finalized || !d->finalized) return fail("model/data not finalized");
   if (!position_worlds || !velocity_worlds) return fail("mjb_team_residency: null output");
   if (check(resident_worlds_position(m->dev, d->dev, position_worlds), "resident_worlds_position")) return -1;
-  if (check(resident_worlds_velocity(m->dev, d->dev, velocity_worlds), "resident_worlds_velocity")) return -1;
+  if (check(resident_worlds_velocity(m->dev, d->dev, velocity_worlds, fluid(m, d)), "resident_worlds_velocity")) return -1;
   return 0;
 }
 int mjb_ctrl_noise(const mjbModel* m, mjbData* d, const float* ctrl_center, int step, float noise_std, float noise_rate, void* stream) {

@@ -21,9 +21,9 @@ __host__ __device__ inline int int_words(const ModelDev& m) {
   return (o + 3) & ~3;
 }
 
-template <bool BAT>
-__global__ void __launch_bounds__(32)
-k_euler(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d, int integrator) {
+// FLUID: implicitfast includes the fluid force derivatives (k_euler_fluid)
+template <bool FLUID, bool BAT>
+__device__ __forceinline__ void euler(const ModelDev& mp, const DataDev& d, int integrator, const FluidDev& f) {
   extern __shared__ float smem[];
   const int lane = threadIdx.x, warp = 0;  // one warp per block: the world index is block-uniform
   const int w = blockIdx.x + d.w0;
@@ -52,7 +52,7 @@ k_euler(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d, 
 #pragma unroll 1
     for (int t = 0; t < m.ntree; t++) {
       const int start = m.tree_dofadr[t], n = m.tree_dofnum[t], ld = chol_ld(n);
-      tree_implicit_a(m, d, wb, Mw, start, n, ld, dt, implicitfast, damper, A, lane);
+      tree_implicit_a<FLUID>(m, d, wb, Mw, start, n, ld, dt, implicitfast, damper, A, lane, f);
       if (n <= 32) {
         const float b = lane < n ? d.efc_Ma[wb * nv + start + lane] : 0.f;
         const float xx = chol_solve_reg_any(A, ld, n, b, A, ld, lane);
@@ -94,6 +94,15 @@ k_euler(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d, 
     if (d.nacon[0] > d.naconmax) ovf |= OVF_NARROWPHASE;
     if (ovf) d.overflow[w] |= ovf;
   }
+}
+
+template <bool BAT>
+__global__ void __launch_bounds__(32)
+k_euler(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d, int integrator) { euler<false, BAT>(mp, d, integrator, FluidDev{}); }
+template <bool BAT>
+__global__ void __launch_bounds__(32)
+k_euler_fluid(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d, int integrator, const __grid_constant__ FluidDev f) {
+  euler<true, BAT>(mp, d, integrator, f);
 }
 
 // deterministic Halton value (reference util_misc.py:61-76)
@@ -262,7 +271,7 @@ k_rk_stage(const __grid_constant__ ModelDev m, const __grid_constant__ DataDev d
 size_t smem_integrate(const ModelDev& m) { return (size_t)int_words(m) * sizeof(float); }
 
 // integrator: INT_EULER / INT_IMPLICITFAST / INT_IMPLICIT, or -1 for the model's own (RK4 models advance with Euler here, forward.py:1411)
-cudaError_t launch_integrate(const ModelDev& m, const DataDev& d, int integrator, cudaStream_t s) {
+cudaError_t launch_integrate(const ModelDev& m, const DataDev& d, int integrator, cudaStream_t s, const FluidDev& f) {
   if (integrator < 0) integrator = (m.integrator == INT_IMPLICITFAST || m.integrator == INT_IMPLICIT) ? m.integrator : INT_EULER;
   const bool solve = integrator == INT_IMPLICITFAST || integrator == INT_IMPLICIT || !(m.disableflags & (DSBL_EULERDAMP | DSBL_DAMPER));
   cudaError_t e = integrator == INT_IMPLICIT ? launch_implicit_solve(m, d, d.imp_qacc, s) : cudaSuccess;
@@ -271,7 +280,8 @@ cudaError_t launch_integrate(const ModelDev& m, const DataDev& d, int integrator
     const long n = (long)d.wn * m.njnt;
     e = launch(k_euler_flat, (unsigned)((n + 255) / 256), 256, 0, s, m, d);
   } else {
-    e = launch(m.batched ? k_euler<true> : k_euler<false>, d.wn, 32, smem_integrate(m), s, m, d, integrator);
+    e = f.has_fluid ? launch(m.batched ? k_euler_fluid<true> : k_euler_fluid<false>, d.wn, 32, smem_integrate(m), s, m, d, integrator, f)
+                    : launch(m.batched ? k_euler<true> : k_euler<false>, d.wn, 32, smem_integrate(m), s, m, d, integrator);
   }
   if (e != cudaSuccess || m.na <= 0 || m.nu <= 0) return e;
   const long n = (long)d.wn * m.nu;  // after the integrator kernel: it reads the activations of the step

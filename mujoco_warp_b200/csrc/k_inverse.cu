@@ -50,9 +50,9 @@ __device__ __forceinline__ float row_dot_g(const float* __restrict__ Jr, const f
 
 // disc: convert the given (discrete-time) qacc to continuous time first, qacc <- M^-1 A qacc, and write it to qacc_cont.
 // qfrc_inverse and qacc_cont are arguments, not DataDev fields: a larger DataDev would move every field of every other kernel.
-template <bool ELL, bool BIG, bool BAT>
-__global__ void __launch_bounds__(32)
-k_inverse(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d, float* __restrict__ qfrc_inverse, float* __restrict__ qacc_cont, int disc) {
+// FLUID: the implicitfast conversion includes the fluid force derivatives (k_inverse_fluid)
+template <bool FLUID, bool ELL, bool BIG, bool BAT>
+__device__ __forceinline__ void inverse(const ModelDev& mp, const DataDev& d, float* __restrict__ qfrc_inverse, float* __restrict__ qacc_cont, int disc, const FluidDev& f) {
   extern __shared__ float smem[];
   const int lane = threadIdx.x;  // one warp (one block) owns the world
   const int w = blockIdx.x + d.w0;
@@ -77,7 +77,7 @@ k_inverse(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d
 #pragma unroll 1
     for (int t = 0; t < m.ntree; t++) {
       const int start = m.tree_dofadr[t], n = m.tree_dofnum[t], ld = inv_ld(n);
-      tree_implicit_a(m, d, wb, Mw, start, n, ld, m.timestep, implicitfast, damper, A, lane);
+      tree_implicit_a<FLUID>(m, d, wb, Mw, start, n, ld, m.timestep, implicitfast, damper, A, lane, f);
       __syncwarp();
 #pragma unroll 1
       for (int i = lane; i < n; i += 32) {  // A holds the lower triangle
@@ -161,13 +161,30 @@ k_inverse(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d
   if (lane == 0) d.solver_niter[w] = 0;
 }
 
+template <bool ELL, bool BIG, bool BAT>
+__global__ void __launch_bounds__(32)
+k_inverse(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d, float* __restrict__ qfrc_inverse, float* __restrict__ qacc_cont, int disc) {
+  inverse<false, ELL, BIG, BAT>(mp, d, qfrc_inverse, qacc_cont, disc, FluidDev{});
+}
+template <bool ELL, bool BIG, bool BAT>
+__global__ void __launch_bounds__(32)
+k_inverse_fluid(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d, float* __restrict__ qfrc_inverse, float* __restrict__ qacc_cont, int disc,
+                const __grid_constant__ FluidDev f) {
+  inverse<true, ELL, BIG, BAT>(mp, d, qfrc_inverse, qacc_cont, disc, f);
+}
+
 }  // namespace
 
-// Instantiated by what the model can produce: elliptic cones, nv > 32 (more than one dof per lane), per-world (batched) fields.
-cudaError_t launch_inverse(const ModelDev& m, const DataDev& d, float* qfrc_inverse, float* qacc_cont, bool disc, cudaStream_t s) {
+// Instantiated by what the model can produce: elliptic cones, nv > 32 (more than one dof per lane), per-world (batched) fields, fluid forces.
+cudaError_t launch_inverse(const ModelDev& m, const DataDev& d, float* qfrc_inverse, float* qacc_cont, bool disc, cudaStream_t s, const FluidDev& f) {
   const int which = 4 * (m.batched ? 1 : 0) + 2 * (m.nv > 32 ? 1 : 0) + (m.cone == CONE_ELLIPTIC ? 1 : 0);
   static void (*const kerns[8])(ModelDev, DataDev, float*, float*, int) = {
     k_inverse<false, false, false>, k_inverse<true, false, false>, k_inverse<false, true, false>, k_inverse<true, true, false>,
     k_inverse<false, false, true>,  k_inverse<true, false, true>,  k_inverse<false, true, true>,  k_inverse<true, true, true>};
-  return launch(kerns[which], d.wn, 32, (size_t)inv_layout(m, d, disc).total * sizeof(float), s, m, d, qfrc_inverse, qacc_cont, (int)disc);
+  static void (*const kerns_fluid[8])(ModelDev, DataDev, float*, float*, int, FluidDev) = {
+    k_inverse_fluid<false, false, false>, k_inverse_fluid<true, false, false>, k_inverse_fluid<false, true, false>, k_inverse_fluid<true, true, false>,
+    k_inverse_fluid<false, false, true>,  k_inverse_fluid<true, false, true>,  k_inverse_fluid<false, true, true>,  k_inverse_fluid<true, true, true>};
+  const size_t smem = (size_t)inv_layout(m, d, disc).total * sizeof(float);
+  if (f.has_fluid) return launch(kerns_fluid[which], d.wn, 32, smem, s, m, d, qfrc_inverse, qacc_cont, (int)disc, f);
+  return launch(kerns[which], d.wn, 32, smem, s, m, d, qfrc_inverse, qacc_cont, (int)disc);
 }

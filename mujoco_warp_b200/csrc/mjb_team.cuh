@@ -111,8 +111,10 @@ struct Stager {
 // ---------------------------------------------------------------- host side: shape, configuration and launch of a team kernel
 // A team kernel (k_position, k_velocity) is one instance per lanes-per-world count, `kernel_of(m, lpw)`, taking (m, d, stage mask),
 // with `world_words` floats of shared memory per world.
+// Instances may take arguments after the mask (the fluid instances of k_velocity), so the chooser's kernel type is a parameter.
 using TeamKernel = void (*)(ModelDev, DataDev, int);
-using TeamChooser = TeamKernel (*)(const ModelDev& m, int lpw);
+template <class K>
+using TeamChooserOf = K (*)(const ModelDev& m, int lpw);
 
 // Launch shape of a team kernel: lanes per world and warps per block, from the per-world shared-memory footprint.
 // Default 8 lanes per world (4 worlds per warp); models whose worlds are too large for that fall back to fewer worlds per warp.
@@ -122,7 +124,8 @@ using TeamChooser = TeamKernel (*)(const ModelDev& m, int lpw);
 // instance for lpw), block and warp limits allow; ties go to two-warp blocks.  Batched models have only a 32-lane instance:
 // where the footprint alone would give fewer lanes per world, they take 32 lanes in two-warp blocks.
 struct TeamShape { int lpw, wpb; size_t block_bytes; };
-inline TeamShape team_shape(const ModelDev& m, int nworld, size_t world_words, TeamChooser kernel_of) {
+template <class K>
+inline TeamShape team_shape(const ModelDev& m, int nworld, size_t world_words, TeamChooserOf<K> kernel_of) {
   constexpr size_t kBlockMax = 200 * 1024;  // leaves room for a second resident block's reserve
   auto bytes = [&](int lpw) { return (world_words * (size_t)(32 / lpw) + 4) * sizeof(float); };
   int lpw = 8;
@@ -159,16 +162,18 @@ inline int team_carveout(size_t block_bytes) {
   return pct < 100 ? (int)pct : (int)cudaSharedmemCarveoutMaxShared;
 }
 
-inline cudaError_t team_launch(const ModelDev& m, const DataDev& d, size_t world_words, TeamChooser kernel_of, int mask, cudaStream_t s) {
+template <class K, class... A>
+inline cudaError_t team_launch(const ModelDev& m, const DataDev& d, size_t world_words, TeamChooserOf<K> kernel_of, int mask, cudaStream_t s, const A&... extra) {
   const TeamShape t = team_shape(m, d.wn, world_words, kernel_of);
   const int G = 32 / t.lpw, ngroups = (d.wn + G - 1) / G, grid = (ngroups + t.wpb - 1) / t.wpb;
-  return launch(kernel_of(m, t.lpw), grid, 32 * t.wpb, t.block_bytes, team_carveout(t.block_bytes), s, m, d, mask);
+  return launch(kernel_of(m, t.lpw), grid, 32 * t.wpb, t.block_bytes, team_carveout(t.block_bytes), s, m, d, mask, extra...);
 }
 
 // Worlds per SM resident at once (occupancy API) in the launch shape of d's world range.
-inline cudaError_t team_resident_worlds(const ModelDev& m, const DataDev& d, size_t world_words, TeamChooser kernel_of, int* worlds) {
+template <class K>
+inline cudaError_t team_resident_worlds(const ModelDev& m, const DataDev& d, size_t world_words, TeamChooserOf<K> kernel_of, int* worlds) {
   const TeamShape t = team_shape(m, d.wn, world_words, kernel_of);
-  const TeamKernel kern = kernel_of(m, t.lpw);
+  const K kern = kernel_of(m, t.lpw);
   int blocks = 0;
   cudaError_t e = launch_configure((const void*)kern, t.block_bytes, team_carveout(t.block_bytes));
   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, 32 * t.wpb, t.block_bytes);

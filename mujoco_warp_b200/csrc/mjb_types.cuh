@@ -111,6 +111,24 @@ struct DataDev {
   float* imp_qacc;    // (nworld, nv) acceleration solved by the fully implicit integrator (k_implicit.cu), consumed by the advance kernel
 };
 
+// ---------------------------------------------------------------- fluid forces (mjb_fluid.cuh)
+// Model and Data fields of fluid forces, passed as one extra argument to the fluid instances of k_velocity, k_euler and k_inverse only:
+// adding them to ModelDev / DataDev would move the kernel parameters of every other kernel.  density / viscosity / wind are model
+// constants (the reference indexes them per world).
+#define MJB_FLUID_INTS(X) X(has_fluid)
+#define MJB_FLUID_FLOATS(X) X(density) X(viscosity) X(wind_x) X(wind_y) X(wind_z)
+#define MJB_FLUID_IARRS(X) X(body_fluid) X(body_geomadr) X(body_geomnum)
+#define MJB_FLUID_FARRS(X) X(geom_fluid)
+struct FluidDev {
+  int has_fluid;                         // opt.density > 0, opt.viscosity > 0 or a non-zero opt.wind
+  float density, viscosity, wind_x, wind_y, wind_z;
+  const int* __restrict__ body_fluid;    // (nbody) FLUID_NONE / FLUID_ELLIPSOID / FLUID_BOX
+  const int* __restrict__ body_geomadr;  // (nbody)
+  const int* __restrict__ body_geomnum;  // (nbody)
+  const float* __restrict__ geom_fluid;  // (ngeom, 12), MuJoCo's layout
+  float* __restrict__ qfrc_fluid;        // Data.qfrc_fluid (nworld, nv)
+};
+
 // ---------------------------------------------------------------- enums (MuJoCo values; see constants.py)
 enum { JNT_FREE = 0, JNT_BALL = 1, JNT_SLIDE = 2, JNT_HINGE = 3 };
 enum { GEOM_PLANE = 0, GEOM_HFIELD, GEOM_SPHERE, GEOM_CAPSULE, GEOM_ELLIPSOID, GEOM_CYLINDER, GEOM_BOX, GEOM_MESH };
@@ -160,18 +178,18 @@ size_t smem_collision_mesh(const ModelDev& m, const DataDev& d);
 cudaError_t reset_contact_counters(const DataDev& d, cudaStream_t s);
 cudaError_t launch_constraint(const ModelDev& m, const DataDev& d, cudaStream_t s);
 cudaError_t launch_efc_csr(const ModelDev& m, const DataDev& d, cudaStream_t s);  // CSR view of efc.J (sparse models)
-cudaError_t launch_velocity(const ModelDev& m, const DataDev& d, int stage_mask, cudaStream_t s);
+cudaError_t launch_velocity(const ModelDev& m, const DataDev& d, int stage_mask, cudaStream_t s, const FluidDev& f);
 cudaError_t launch_solve_m(const ModelDev& m, const DataDev& d, float* x, const float* y, cudaStream_t s);
 cudaError_t launch_mul_m(const ModelDev& m, const DataDev& d, float* res, const float* vec, cudaStream_t s);
 cudaError_t launch_solver(const ModelDev& m, const DataDev& d, cudaStream_t s);
-cudaError_t launch_integrate(const ModelDev& m, const DataDev& d, int integrator, cudaStream_t s);
+cudaError_t launch_integrate(const ModelDev& m, const DataDev& d, int integrator, cudaStream_t s, const FluidDev& f);
 cudaError_t launch_implicit_solve(const ModelDev& m, const DataDev& d, float* qacc_out, cudaStream_t s);  // fully implicit integrator: qLU and its solve
 size_t smem_implicit(const ModelDev& m);
 cudaError_t launch_sensor(const ModelDev& m, const DataDev& d, int stages, cudaStream_t s);
 cudaError_t launch_contact_force(const ModelDev& m, const DataDev& d, const int* contact_ids, int n, int to_world, float* out, cudaStream_t s);
 // inverse dynamics at the given d.qacc into qfrc_inverse (nworld, nv); disc: d.qacc is a discrete-time acceleration, converted first,
 // and the continuous one goes to qacc_cont (nworld, nv) (k_inverse.cu)
-cudaError_t launch_inverse(const ModelDev& m, const DataDev& d, float* qfrc_inverse, float* qacc_cont, bool disc, cudaStream_t s);
+cudaError_t launch_inverse(const ModelDev& m, const DataDev& d, float* qfrc_inverse, float* qacc_cont, bool disc, cudaStream_t s, const FluidDev& f);
 cudaError_t launch_rk_stage(const ModelDev& m, const DataDev& d, float* rk, int stage, cudaStream_t s);
 // rays (nworld x nray, world-major) against every geom of every world; geomgroup: 6 ints, all -1 = no group filter (k_ray.cu)
 cudaError_t launch_ray(const ModelDev& m, const DataDev& d, const float* pnt, const float* vec, int nray, int pnt_nbatch, const int* geomgroup, int flg_static,
@@ -180,9 +198,9 @@ cudaError_t launch_ctrl_noise(const ModelDev& m, const DataDev& d, const float* 
 size_t smem_position(const ModelDev& m, const DataDev& d);
 size_t smem_collision(const ModelDev& m, const DataDev& d);
 size_t smem_constraint(const ModelDev& m, const DataDev& d);
-size_t smem_velocity(const ModelDev& m, const DataDev& d);
+size_t smem_velocity(const ModelDev& m, const DataDev& d, const FluidDev& f);
 // worlds per SM resident at once (occupancy API) in the launch shape k_position / k_velocity take for d's world range
 cudaError_t resident_worlds_position(const ModelDev& m, const DataDev& d, int* worlds);
-cudaError_t resident_worlds_velocity(const ModelDev& m, const DataDev& d, int* worlds);
+cudaError_t resident_worlds_velocity(const ModelDev& m, const DataDev& d, int* worlds, const FluidDev& f);
 size_t smem_solver(const ModelDev& m, const DataDev& d);
 size_t smem_integrate(const ModelDev& m);

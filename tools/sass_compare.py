@@ -3,8 +3,8 @@
   python tools/sass_compare.py parent.sass new.sass
 
 Each dump is the concatenated `cuobjdump -sass` of the cubins of one tree (nvcc -cubin -gencode arch=compute_90a,code=sm_90a with the
-flags of _lib.NVCC_FLAGS, one .cu at a time).  The anonymous-namespace hash in the mangled names depends on the file's contents, so it
-is normalised; instructions are compared without their addresses and encodings.  Functions present in only one dump are listed
+flags of _lib.NVCC_FLAGS, one .cu at a time).  The anonymous-namespace hashes in the mangled names (both the prefix and the one after the file name) depend on the file's
+contents, so they are normalised; instructions are compared without their addresses and encodings.  Functions present in only one dump are listed
 (a new kernel is expected there); every function present in both must be identical.
 """
 import re, sys
@@ -13,7 +13,7 @@ def funcs(path):
     for line in open(path):
         m = re.search(r'Function : (\S+)', line)
         if m:
-            cur = re.sub(r'_GLOBAL__N__[0-9a-f]+_', '_GLOBAL__N__X_', m.group(1)); out[cur] = []; continue
+            cur = re.sub(r'(_GLOBAL__N__X_\d+_\w+?_cu_)[0-9a-f]{8}', r'\1X', re.sub(r'_GLOBAL__N__[0-9a-f]+_', '_GLOBAL__N__X_', m.group(1))); out[cur] = []; continue
         if cur is None: continue
         m = re.match(r'\s*/\*([0-9a-f]{4,})\*/\s*(.*?);', line)
         if m: out[cur].append(m.group(2).strip())

@@ -255,6 +255,9 @@ def _build_warp():
   wp.matrix_from_rows = lambda *rows: _mat_cls(len(rows), len(rows[0].v))._from_rows([list(r.v) for r in rows])
   wp.matrix_from_cols = lambda *cols: wp.transpose(wp.matrix_from_rows(*cols))
   wp.identity = lambda n, dtype=float: _mat_cls(n, n)._from_rows([[1.0 if i == j else 0.0 for j in range(n)] for i in range(n)])
+  # the fluid force derivatives (derivative.py:588-852)
+  wp.skew = lambda v: _mat_cls(3, 3)._from_rows([[0.0, -v[2], v[1]], [v[2], 0.0, -v[0]], [-v[1], v[0], 0.0]])
+  wp.outer = lambda a, b: _mat_cls(len(a.v), len(b.v))._from_rows([[p * q for q in b.v] for p in a.v])
   return wp
 
 
