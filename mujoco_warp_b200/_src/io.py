@@ -281,6 +281,58 @@ def derive_tables(mjm) -> dict:
   return t
 
 
+_COLLISION_SENSORS = (C.SENS_GEOMDIST, C.SENS_GEOMNORMAL, C.SENS_GEOMFROMTO)
+
+
+def _sensor_collision_tables(mjm, t) -> dict:
+  """The geom pairs of the distance / normal / fromto sensors (reference io.py:586-628), kept apart from nxn_pairid.
+
+  sensor_collision_start_adr: for every (sensor, geom1, geom2) in the sensors' loop order (body sensors expand over body_geomadr /
+  body_geomnum), the index of that geom pair among the nsensorcollision unique pairs, numbered in first-seen order.  The kernel's own tables:
+  sensor_collision_pair (nsensorcollision, 4): both geoms in the order the narrowphase takes them (geom types ascending) and the pair's
+  explicit <pair> id or -1 (its margin), and the pair's rank among the pairs that run GJK / EPA or -1 (its scratch slot); sensor_collision_id / _adr: the collision sensors and their first entry of the start_adr list;
+  sensor_collision_flip: whether an entry's geom1 comes second in narrowphase order (the reduction then reverses normal and fromto)."""
+  nsensor, ngeom = int(getattr(mjm, "nsensor", 0)), int(mjm.ngeom)
+  stype = np.asarray(mjm.sensor_type).reshape(-1) if nsensor else np.zeros(0, dtype=int)
+  sensors = np.nonzero(np.isin(stype, _COLLISION_SENSORS))[0]
+  gt, gadr, gnum = _np(mjm, "geom_type"), _np(mjm, "body_geomadr"), _np(mjm, "body_geomnum")
+
+  def geoms(objtype, objid):
+    return range(int(gadr[objid]), int(gadr[objid] + gnum[objid])) if objtype == C.OBJ_BODY else range(int(objid), int(objid) + 1)
+
+  nativeccd = not (int(mjm.opt.disableflags) & C.DSBL_NATIVECCD)
+  is_ccd = lambda key: key in _CONVEX_PAIRS or (key == (C.GEOM_BOX, C.GEOM_BOX) and nativeccd)
+  nccd = 0
+  first = {}  # upper-triangular pair index -> collision id
+  pairs, start_adr, flip, adr = [], [], [], []
+  for s in sensors:
+    adr.append(len(start_adr))
+    for g1 in geoms(int(mjm.sensor_objtype[s]), int(mjm.sensor_objid[s])):
+      for g2 in geoms(int(mjm.sensor_reftype[s]), int(mjm.sensor_refid[s])):
+        a, b = min(g1, g2), max(g1, g2)
+        idx = (a * (2 * ngeom - a - 3)) // 2 + b - 1
+        if idx not in first:
+          key = (min(gt[a], gt[b]), max(gt[a], gt[b]))
+          if a == b or not (key in _SUPPORTED_PAIRS or key in _CONVEX_PAIRS or key == (C.GEOM_BOX, C.GEOM_BOX)):
+            names = ("plane", "hfield", "sphere", "capsule", "ellipsoid", "cylinder", "box", "mesh", "sdf")
+            raise NotImplementedError(f"collision sensor {s}: no collider for the geom types {names[key[0]]} and {names[key[1]]} (geoms {a} and {b})")
+          first[idx] = len(pairs)
+          lo, hi = (b, a) if gt[a] > gt[b] else (a, b)
+          pairs.append((lo, hi, int(t["nxn_pairid"][idx, 0]) if t["nxn_pairid"][idx, 0] >= 0 else -1, nccd if is_ccd(key) else -1))
+          nccd += is_ccd(key)
+        start_adr.append(first[idx])
+        flip.append(int(gt[g1] > gt[g2] or (gt[g1] == gt[g2] and g1 > g2)))
+  adr.append(len(start_adr))
+  # EPA iterations as the reference counts them over its pair list, which includes the sensor pairs (collision_convex.py:1223)
+  convex = [(min(gt[a], gt[b]), max(gt[a], gt[b])) for a, b in list(t["nxn_geom_pair_filtered"]) + [p[:2] for p in pairs]]
+  convex = [k for k in convex if is_ccd(k)]
+  epa = 16 if all(k == (C.GEOM_BOX, C.GEOM_BOX) for k in convex) else int(getattr(mjm.opt, "ccd_iterations", 35))
+  i32 = lambda x, shape: np.asarray(x, dtype=np.int32).reshape(shape)
+  return dict(nsensorcollision=len(pairs), sensor_collision_start_adr=i32(start_adr, -1), sensor_collision_pair=i32(pairs, (len(pairs), 4)),
+              sensor_collision_id=i32(sensors, -1), sensor_collision_adr=i32(adr, -1), sensor_collision_flip=i32(flip, -1), sensor_collision_epa_iterations=epa,
+              nsensorcollision_ccd=nccd)
+
+
 def _has_fluid(o) -> bool:
   """io.py:471: the model has fluid forces."""
   return bool(np.any(np.asarray(getattr(o, "wind", 0.0)) != 0.0) or float(getattr(o, "density", 0.0)) > 0.0 or float(getattr(o, "viscosity", 0.0)) > 0.0)
@@ -480,6 +532,10 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   stype = np.asarray(mjm.sensor_type) if nsensor else np.zeros(0, dtype=int)
   m.sensor_subtree_vel = bool(np.isin(stype, (C.SENS_SUBTREELINVEL, C.SENS_SUBTREEANGMOM)).any())  # reference io.py:896-897
   m.sensor_rne_postconstraint = bool(np.isin(stype, (C.SENS_ACCELEROMETER, C.SENS_FORCE, C.SENS_TORQUE, C.SENS_FRAMELINACC, C.SENS_FRAMEANGACC)).any())  # :900
+  sc = _sensor_collision_tables(mjm, t)
+  m.nsensorcollision, m.sensor_collision_epa_iterations, m.nsensorcollision_ccd = (sc.pop(k) for k in ("nsensorcollision", "sensor_collision_epa_iterations", "nsensorcollision_ccd"))
+  for n, x in sc.items():
+    setattr(m, n, dev_i(x))
   m.eq_type = dev_i(mjm.eq_type if neq else np.zeros(0))
   m.eq_obj1id = dev_i(mjm.eq_obj1id if neq else np.zeros(0))
   m.eq_obj2id = dev_i(mjm.eq_obj2id if neq else np.zeros(0))
@@ -556,6 +612,9 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   )
   for k, v in ints.items():
     _lib.check(L.mjb_model_set_int(h, k.encode(), int(v)))
+  for k, v in (("nsensorcollision", m.nsensorcollision), ("nsensorcollision_sensor", len(m.sensor_collision_id)), ("sensor_collision_epa_iterations", m.sensor_collision_epa_iterations),
+               ("nsensorcollision_ccd", m.nsensorcollision_ccd)):
+    _lib.check(L.mjb_model_set_int(h, k.encode(), int(v)))
   g = np.asarray(o.gravity, dtype=np.float64)
   floats = dict(timestep=o.timestep, tolerance=tol, ls_tolerance=o.ls_tolerance, impratio_invsqrt=1.0 / np.sqrt(o.impratio),
                 meaninertia=mjm.stat.meaninertia, gravity_x=g[0], gravity_y=g[1], gravity_z=g[2], ccd_tolerance=float(getattr(o, "ccd_tolerance", 1e-6)))
@@ -578,7 +637,8 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
                                          "actuator_actlimited", "actuator_actearly", "actuator_dynprm", "actuator_actrange", "actuator_trntype",
                                          "ten_J_rownnz", "ten_J_rowadr", "ten_J_colind", "tendon_adr", "tendon_num", "wrap_objid", "tendon_limited", "tendon_actfrclimited", "wrap_prm", "ten_J0",
                                          "geom_group", "geom_matid", "geom_rgba", "mat_rgba", "mesh_faceadr", "mesh_face",
-                                         "geom_fluid", "body_fluid", "body_geomadr", "body_geomnum"]
+                                         "geom_fluid", "body_fluid", "body_geomadr", "body_geomnum", "sensor_collision_start_adr", "sensor_collision_pair",
+                                         "sensor_collision_id", "sensor_collision_adr", "sensor_collision_flip"]
                                         + [n for n, _ in _TENDON_FLOATS]):
     dev_names.setdefault(n, getattr(m, n))
   for n, x in dev_names.items():

@@ -1456,6 +1456,8 @@ def compile_xml(root):
     "framezaxis": (S.SENS_FRAMEZAXIS, "obj", 3, 2, 1),
     "framequat": (S.SENS_FRAMEQUAT, "obj", 4, 3, 1), "framelinvel": (S.SENS_FRAMELINVEL, "obj", 3, 0, 2), "frameangvel": (S.SENS_FRAMEANGVEL, "obj", 3, 0, 2),
     "framelinacc": (S.SENS_FRAMELINACC, "obj", 3, 0, 3), "frameangacc": (S.SENS_FRAMEANGACC, "obj", 3, 0, 3),
+    # collision sensors between two geoms or bodies: signed distance, unit normal (AXIS), and the two witness points
+    "distance": (S.SENS_GEOMDIST, "pair", 1, 0, 1), "normal": (S.SENS_GEOMNORMAL, "pair", 3, 2, 1), "fromto": (S.SENS_GEOMFROMTO, "pair", 6, 0, 1),
   }
   objkind = {"tendon": (C.OBJ_TENDON, "tendon"), "joint": (C.OBJ_JOINT, "joint"), "actuator": (C.OBJ_ACTUATOR, "actuator"), "site": (C.OBJ_SITE, "site"), "body": (C.OBJ_BODY, "body")}
   objtypes = {"body": (C.OBJ_BODY, "body"), "xbody": (C.OBJ_XBODY, "body"), "geom": (C.OBJ_GEOM, "geom"), "site": (C.OBJ_SITE, "site"), "camera": (C.OBJ_CAMERA, "camera")}
@@ -1473,6 +1475,15 @@ def compile_xml(root):
       rid = getattr(m.names, rlst).index(e.get("refname"))
     if kind is None:
       otype, oid = C.OBJ_UNKNOWN, -1
+    elif kind == "pair":  # exactly one of geom<k> / body<k> for each side; the second side is the reference object
+      sides = []
+      for k in ("1", "2"):
+        given = [x for x in ("geom", "body") if x + k in e.attrib]
+        if len(given) != 1:
+          raise ValueError(f"{e.tag} sensor '{e.get('name', f'sensor{len(sens)}')}': give exactly one of geom{k} / body{k}")
+        otype_k, lst = objtypes[given[0]]
+        sides.append((otype_k, getattr(m.names, lst).index(e.get(given[0] + k))))
+      (otype, oid), (rtype, rid) = sides
     elif kind == "obj":
       otype, lst = objtypes[e.get("objtype")]
       oid = getattr(m.names, lst).index(e.get("objname"))

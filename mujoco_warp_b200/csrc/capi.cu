@@ -13,6 +13,7 @@ using std::min;
 struct mjbModel {
   ModelDev dev;
   FluidDev fluid;  // qfrc_fluid stays null here: it is the Data's (fluid() below)
+  SensorCollisionDev sc;
   bool finalized;
 };
 struct mjbData {
@@ -53,6 +54,7 @@ mjbModel* mjb_model_create(void) {
   mjbModel* m = new mjbModel();
   memset(&m->dev, 0, sizeof(ModelDev));
   memset(&m->fluid, 0, sizeof(FluidDev));
+  memset(&m->sc, 0, sizeof(SensorCollisionDev));
   m->finalized = false;
   return m;
 }
@@ -64,6 +66,9 @@ int mjb_model_set_int(mjbModel* m, const char* name, int v) {
 #undef X
 #define X(n) if (!strcmp(name, #n)) { m->fluid.n = v; return 0; }
   MJB_FLUID_INTS(X)
+#undef X
+#define X(n) if (!strcmp(name, #n)) { m->sc.n = v; return 0; }
+  MJB_SENSCOL_INTS(X)
 #undef X
   return fail(std::string("unknown model int field: ") + name);
 }
@@ -84,6 +89,9 @@ int mjb_model_set_array_batched(mjbModel* m, const char* name, const void* p, in
 #define X(n) if (!strcmp(name, #n)) { if (nbatch != 1) return fail(std::string("shared by all worlds (not batched): ") + name); m->fluid.n = (decltype(m->fluid.n))p; return 0; }
   MJB_FLUID_IARRS(X)
   MJB_FLUID_FARRS(X)
+#undef X
+#define X(n) if (!strcmp(name, #n)) { if (nbatch != 1) return fail(std::string("shared by all worlds (not batched): ") + name); m->sc.n = (const int*)p; return 0; }
+  MJB_SENSCOL_IARRS(X)
 #undef X
 #define X(n) if (!strcmp(name, #n)) { m->dev.n = (const float*)p; m->dev.nb_##n = nbatch; m->dev.bs_##n = batch_stride; goto done; }
   MJB_MODEL_FARRS(X)
@@ -108,6 +116,9 @@ int mjb_model_finalize(mjbModel* m) {
 #define X(n) if (!m->fluid.n) return fail(std::string("model array not set: ") + #n);
   MJB_FLUID_IARRS(X)
   MJB_FLUID_FARRS(X)
+#undef X
+#define X(n) if (!m->sc.n) return fail(std::string("model array not set: ") + #n);
+  MJB_SENSCOL_IARRS(X)
 #undef X
   if (m->dev.nv <= 0 || m->dev.nbody <= 0) return fail("model has no dofs/bodies");
   if (m->dev.solver != SOL_NEWTON && m->dev.solver != SOL_CG) return fail("only the Newton and CG solvers are implemented");
@@ -187,6 +198,12 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
       snprintf(buf, sizeof buf, "%s kernel needs %zu B of shared memory per block (> %zu): model/njmax too large for this version", names[i], smem[i], kMaxSmem);
       return fail(buf);
     }
+  if (smem_sensor_collision(m->sc) > kMaxSmem) {
+    char buf[200];
+    snprintf(buf, sizeof buf, "collision-sensor kernel needs %zu B of shared memory per block (> %zu): too many sensor geom pairs or GJK / EPA iterations",
+             smem_sensor_collision(m->sc), kMaxSmem);
+    return fail(buf);
+  }
   {
     const char* e = getenv("MJB_SPLIT");
     const int want = e ? atoi(e) : 2;
@@ -258,9 +275,9 @@ int mjb_rays(const mjbModel* m, mjbData* d, const float* pnt, const float* vec, 
   MJB_LAUNCH(launch_ray(m->dev, d->dev, pnt, vec, nray, pnt_nbatch, geomgroup, flg_static, bodyexclude, dist, geomid, normal, s));
   return 0;
 }
-int mjb_sensor_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 1, s)); return 0; }
-int mjb_sensor_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 2, s)); return 0; }
-int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 4, s)); return 0; }
+int mjb_sensor_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 1, s, m->sc)); return 0; }
+int mjb_sensor_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 2, s, m->sc)); return 0; }
+int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 4, s, m->sc)); return 0; }
 int mjb_solve(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_solver(m->dev, d->dev, s)); return 0; }
 int mjb_euler(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_integrate(m->dev, d->dev, INT_EULER, s, fluid(m, d))); return 0; }
 
@@ -295,7 +312,7 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
   if (what & RUN_SOLVER) {
     MJB_LAUNCH(launch_solver(m->dev, dd, s));
     // sensors of all three stages in one launch after the solver (forward.py:1350-1365 interleaves them; their inputs are final by now)
-    if (m->dev.nsensor > 0) MJB_LAUNCH(launch_sensor(m->dev, dd, 7, s));
+    if (m->dev.nsensor > 0) MJB_LAUNCH(launch_sensor(m->dev, dd, 7, s, m->sc));
     MJB_MARK(4);
   }
   if (what & RUN_INVERSE) {
@@ -306,7 +323,7 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
     if (m->dev.nsensor > 0) {
       DataDev ds = dd;
       if (disc) ds.qacc = d->inv_qacc;
-      MJB_LAUNCH(launch_sensor(m->dev, ds, 7, s));
+      MJB_LAUNCH(launch_sensor(m->dev, ds, 7, s, m->sc));
     }
   }
   if (what & RUN_EULER) {

@@ -359,7 +359,10 @@ k_sensor(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d,
 
 }  // namespace
 
-cudaError_t launch_sensor(const ModelDev& m, const DataDev& d, int stages, cudaStream_t s) {
+cudaError_t launch_sensor(const ModelDev& m, const DataDev& d, int stages, cudaStream_t s, const SensorCollisionDev& c) {
   if (m.nsensor == 0) return cudaSuccess;
-  return launch(m.batched ? k_sensor<true> : k_sensor<false>, d.wn, 32, (size_t)12 * m.nbody * sizeof(float), s, m, d, stages);
+  const cudaError_t e = launch(m.batched ? k_sensor<true> : k_sensor<false>, d.wn, 32, (size_t)12 * m.nbody * sizeof(float), s, m, d, stages);
+  // k_sensor skips the collision sensors: their slots are k_sensor_collision's
+  if (e != cudaSuccess || !(stages & STAGE_POS) || c.nsensorcollision == 0 || (m.disableflags & DSBL_SENSOR)) return e;
+  return launch_sensor_collision(m, d, c, s);
 }

@@ -114,6 +114,24 @@ struct Polytope {
   int* vidx;         // 5 + it: box corner ids of each support pair (geom1 | geom2 << 4)
 };
 
+#if CCD_MESH
+// collision_core.py:60-140 geom(): a mesh geom carries its asset's vertex block, hull graph and hull polygon tables
+static __device__ __forceinline__ void fill_mesh(const ModelDev& m, int g, CGeom& c) {
+  c.index = -1; c.vertnum = 0; c.polynum = 0; c.vert = nullptr; c.polynormal = nullptr; c.graph = nullptr;
+  c.polyvertadr = c.polyvertnum = c.polyvert = c.polymapadr = c.polymapnum = c.polymap = nullptr;
+  if (c.type != GEOM_MESH) return;
+  const int id = m.geom_dataid[g];
+  if (id < 0) return;
+  const int vadr = m.mesh_vertadr[id], padr = m.mesh_polyadr[id];
+  c.vert = m.mesh_vert + 3 * vadr; c.vertnum = m.mesh_vertnum[id];
+  c.graph = m.mesh_graphadr[id] >= 0 ? m.mesh_graph + m.mesh_graphadr[id] : nullptr;
+  c.polynum = m.mesh_polynum[id]; c.polynormal = m.mesh_polynormal + 3 * padr;
+  c.polyvertadr = m.mesh_polyvertadr + padr; c.polyvertnum = m.mesh_polyvertnum + padr; c.polyvert = m.mesh_polyvert;
+  c.polymapadr = m.mesh_polymapadr + vadr; c.polymapnum = m.mesh_polymapnum + vadr; c.polymap = m.mesh_polymap;
+}
+
+#endif
+
 static __device__ __forceinline__ float csign(float x) { return x < 0.f ? -1.f : 1.f; }  // wp.sign(0) = +1
 
 #if CCD_MESH

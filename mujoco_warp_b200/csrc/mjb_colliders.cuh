@@ -43,6 +43,37 @@ static __device__ __forceinline__ float col_sphere_sphere(v3 pos1, float r1, v3 
   return dist;
 }
 
+// collision_primitive_core.py capsule_capsule for the collision sensors, the arithmetic k_collision inlines: the closest segment points, or up to two end points of
+// (nearly) parallel segments; only contacts within `margin` are produced (dist INFINITY otherwise)
+static __device__ __forceinline__ void capsule_capsule(v3 pos1, v3 ax1, v3 size1, v3 pos2, v3 ax2, v3 size2, float margin, float* cd, v3* cp, v3* cn) {
+  const v3 axis1 = ax1 * size1.y, axis2 = ax2 * size2.y, dif = pos1 - pos2;
+  const float ma = dot(axis1, axis1), mb = -dot(axis1, axis2), mc = dot(axis2, axis2), u = -dot(axis1, dif), v = dot(axis2, dif);
+  const float det = ma * mc - mb * mb;
+  v3 p, n;
+  if (fabsf(det) >= MJ_MINVAL) {
+    const float inv = 1.0f / det;
+    float x1 = (mc * u - mb * v) * inv, x2 = (ma * v - mb * u) * inv;
+    if (x1 > 1.f) { x1 = 1.f; x2 = (v - mb) / mc; } else if (x1 < -1.f) { x1 = -1.f; x2 = (v + mb) / mc; }
+    if (x2 > 1.f) { x2 = 1.f; x1 = clampf((u - mb) / ma, -1.f, 1.f); } else if (x2 < -1.f) { x2 = -1.f; x1 = clampf((u + mb) / ma, -1.f, 1.f); }
+    const float dist = col_sphere_sphere(pos1 + axis1 * x1, size1.x, pos2 + axis2 * x2, size2.x, &p, &n);
+    if (dist <= margin) { cd[0] = dist; cp[0] = p; cn[0] = n; }
+    return;
+  }
+  int cc = 0;
+  float dist = col_sphere_sphere(pos1 + axis1, size1.x, pos2 + axis2 * clampf((v - mb) / mc, -1.f, 1.f), size2.x, &p, &n);
+  if (dist <= margin) { cd[cc] = dist; cp[cc] = p; cn[cc] = n; cc++; }
+  dist = col_sphere_sphere(pos1 - axis1, size1.x, pos2 + axis2 * clampf((v + mb) / mc, -1.f, 1.f), size2.x, &p, &n);
+  if (dist <= margin) { cd[cc] = dist; cp[cc] = p; cn[cc] = n; cc++; }
+  if (cc < 2) {
+    dist = col_sphere_sphere(pos1 + axis1 * clampf((u - mb) / ma, -1.f, 1.f), size1.x, pos2 + axis2, size2.x, &p, &n);
+    if (dist <= margin) { cd[cc] = dist; cp[cc] = p; cn[cc] = n; cc++; }
+  }
+  if (cc < 2) {
+    dist = col_sphere_sphere(pos1 + axis1 * clampf((u + mb) / ma, -1.f, 1.f), size1.x, pos2 - axis2, size2.x, &p, &n);
+    if (dist <= margin) { cd[cc] = dist; cp[cc] = p; cn[cc] = n; }
+  }
+}
+
 static __device__ __forceinline__ float plane_ellipsoid(v3 n, v3 ppos, v3 epos, const float* erot, v3 esize, v3* pos) {
   const v3 sup = normalize(cw_mul(mat_t_vec(erot, n), esize)) * -1.0f;
   v3 p = epos + matvec(erot, cw_mul(sup, esize));

@@ -129,6 +129,24 @@ struct FluidDev {
   float* __restrict__ qfrc_fluid;        // Data.qfrc_fluid (nworld, nv)
 };
 
+// ---------------------------------------------------------------- collision sensors (k_sensor_collision.cu)
+// The geom pairs of the distance / normal / fromto sensors (io.py _sensor_collision_tables), passed as one extra argument to
+// k_sensor_collision only, for the same reason as FluidDev.  They stay off nxn_pairid: the contact pipeline never sees them.
+#define MJB_SENSCOL_INTS(X) X(nsensorcollision) X(nsensorcollision_sensor) X(nsensorcollision_ccd) X(sensor_collision_epa_iterations)
+#define MJB_SENSCOL_IARRS(X) X(sensor_collision_start_adr) X(sensor_collision_pair) X(sensor_collision_id) X(sensor_collision_adr) X(sensor_collision_flip)
+struct SensorCollisionDev {
+  int nsensorcollision;                                // unique geom pairs
+  int nsensorcollision_sensor;                         // distance / normal / fromto sensors
+  int nsensorcollision_ccd;                            // pairs that run GJK / EPA (one scratch slot each, at most 32 in use)
+  int sensor_collision_epa_iterations;
+  const int* __restrict__ sensor_collision_start_adr;  // (sum over sensors of n1 n2) unique-pair index of each (sensor, geom1, geom2)
+  const int* __restrict__ sensor_collision_pair;       // (nsensorcollision, 4) geoms in narrowphase order, explicit <pair> id or -1,
+                                                       // GJK / EPA rank among the pairs or -1
+  const int* __restrict__ sensor_collision_id;         // (nsensorcollision_sensor) sensor ids
+  const int* __restrict__ sensor_collision_adr;        // (nsensorcollision_sensor + 1) first start_adr entry of each sensor
+  const int* __restrict__ sensor_collision_flip;       // (like start_adr) the entry's geom1 is the narrowphase's second geom
+};
+
 // ---------------------------------------------------------------- enums (MuJoCo values; see constants.py)
 enum { JNT_FREE = 0, JNT_BALL = 1, JNT_SLIDE = 2, JNT_HINGE = 3 };
 enum { GEOM_PLANE = 0, GEOM_HFIELD, GEOM_SPHERE, GEOM_CAPSULE, GEOM_ELLIPSOID, GEOM_CYLINDER, GEOM_BOX, GEOM_MESH };
@@ -141,7 +159,8 @@ enum { OBJ_BODY = 1, OBJ_XBODY = 2, OBJ_GEOM = 5, OBJ_SITE = 6, OBJ_CAMERA = 7 }
 // mjtSensor values of the sensor types carried here (MuJoCo order, as in _src/constants.py)
 enum { SENS_TOUCH = 0, SENS_ACCELEROMETER = 1, SENS_VELOCIMETER = 2, SENS_GYRO = 3, SENS_FORCE = 4, SENS_TORQUE = 5, SENS_JOINTPOS = 9, SENS_JOINTVEL = 10, SENS_TENDONPOS = 11, SENS_TENDONVEL = 12, SENS_ACTUATORPOS = 13, SENS_ACTUATORVEL = 14,
        SENS_ACTUATORFRC = 15, SENS_JOINTACTFRC = 16, SENS_BALLQUAT = 18, SENS_BALLANGVEL = 19, SENS_JOINTLIMITPOS = 20, SENS_JOINTLIMITVEL = 21, SENS_JOINTLIMITFRC = 22, SENS_FRAMEPOS = 26, SENS_FRAMEQUAT = 27, SENS_FRAMEXAXIS = 28,
-       SENS_FRAMEYAXIS = 29, SENS_FRAMEZAXIS = 30, SENS_FRAMELINVEL = 31, SENS_FRAMEANGVEL = 32, SENS_FRAMELINACC = 33, SENS_FRAMEANGACC = 34, SENS_SUBTREECOM = 35, SENS_SUBTREELINVEL = 36, SENS_SUBTREEANGMOM = 37, SENS_CLOCK = 45 };
+       SENS_FRAMEYAXIS = 29, SENS_FRAMEZAXIS = 30, SENS_FRAMELINVEL = 31, SENS_FRAMEANGVEL = 32, SENS_FRAMELINACC = 33, SENS_FRAMEANGACC = 34, SENS_SUBTREECOM = 35, SENS_SUBTREELINVEL = 36, SENS_SUBTREEANGMOM = 37, SENS_GEOMDIST = 39, SENS_GEOMNORMAL = 40,
+       SENS_GEOMFROMTO = 41, SENS_CLOCK = 45 };
 enum { CNSTR_EQUALITY = 0, CNSTR_FRICTION_DOF = 1, CNSTR_FRICTION_TENDON = 2, CNSTR_LIMIT_JOINT = 3, CNSTR_LIMIT_TENDON = 4, CNSTR_CONTACT_FRICTIONLESS = 5, CNSTR_CONTACT_PYRAMIDAL = 6, CNSTR_CONTACT_ELLIPTIC = 7 };
 enum { ST_SATISFIED = 0, ST_QUADRATIC = 1, ST_LINEARNEG = 2, ST_LINEARPOS = 3, ST_CONE = 4 };
 enum { CAM_FIXED = 0, CAM_TRACK, CAM_TRACKCOM, CAM_TARGETBODY, CAM_TARGETBODYCOM };
@@ -185,7 +204,10 @@ cudaError_t launch_solver(const ModelDev& m, const DataDev& d, cudaStream_t s);
 cudaError_t launch_integrate(const ModelDev& m, const DataDev& d, int integrator, cudaStream_t s, const FluidDev& f);
 cudaError_t launch_implicit_solve(const ModelDev& m, const DataDev& d, float* qacc_out, cudaStream_t s);  // fully implicit integrator: qLU and its solve
 size_t smem_implicit(const ModelDev& m);
-cudaError_t launch_sensor(const ModelDev& m, const DataDev& d, int stages, cudaStream_t s);
+// the sensors of `stages` (1 pos, 2 vel, 4 acc); with the position stage also the collision sensors (k_sensor_collision.cu)
+cudaError_t launch_sensor(const ModelDev& m, const DataDev& d, int stages, cudaStream_t s, const SensorCollisionDev& c);
+cudaError_t launch_sensor_collision(const ModelDev& m, const DataDev& d, const SensorCollisionDev& c, cudaStream_t s);
+size_t smem_sensor_collision(const SensorCollisionDev& c);
 cudaError_t launch_contact_force(const ModelDev& m, const DataDev& d, const int* contact_ids, int n, int to_world, float* out, cudaStream_t s);
 // inverse dynamics at the given d.qacc into qfrc_inverse (nworld, nv); disc: d.qacc is a discrete-time acceleration, converted first,
 // and the continuous one goes to qacc_cont (nworld, nv) (k_inverse.cu)

@@ -776,7 +776,11 @@ def _wp_div(a, b):
   if isinstance(a, int) and isinstance(b, int) and not isinstance(a, bool):
     q = abs(a) // abs(b)
     return q if (a >= 0) == (b >= 0) else -q
-  return a / b
+  try:
+    return a / b
+  except ZeroDivisionError:  # IEEE floats, as on the device: +-inf, or nan for 0 / 0
+    with _np.errstate(divide="ignore", invalid="ignore"):
+      return float(_np.float64(a) / _np.float64(b))
 
 
 def _wp_mod(a, b):
