@@ -37,6 +37,7 @@
  *                                                      D-structure, LU solve, Data.qLU written; IMPLICITFAST: symmetric M - dt qDeriv, Cholesky;
  *                                                      then advance.  Error for Euler / RK4 models: the scratch is sized per integrator)
  *   mjb_ctrl_noise             <- _src/cli.py:103      _ctrl_noise (harness kernel, untimed in testspeed)
+ *   mjb_set_const              <- _src/set_const.py:613-950 set_const_fixed / set_const_0 / set_const_spring / set_const(m, d, restore)
  *
  * Conventions: plain pointers and sizes only (no torch / warp types).  All array pointers are DEVICE
  * pointers owned by the caller for the lifetime of the handle (borrowed, never freed here).  Layout is
@@ -120,6 +121,22 @@ int mjb_rungekutta4(const mjbModel* m, mjbData* d, void* stream);
 int mjb_solve(const mjbModel* m, mjbData* d, void* stream);
 int mjb_euler(const mjbModel* m, mjbData* d, void* stream);
 int mjb_implicit(const mjbModel* m, mjbData* d, void* stream);
+/* set_const.py:613-950: recompute the Model fields the compiler derives from other Model fields.  parts is a combination of
+ *   MJB_SET_CONST_FIXED   body_subtreemass from body_mass (set_const_fixed);
+ *   MJB_SET_CONST_0       at qpos0: stat.meaninertia, tendon_length0, eq_data (connect / weld), dof_invweight0, body_invweight0,
+ *                         tendon_invweight0, cam_pos0 / poscom0 / mat0, light_pos0 / poscom0 / dir0, actuator_acc0 and the dampratio
+ *                         form of affine-bias actuators in actuator_biasprm[2] (set_const_0);
+ *   MJB_SET_CONST_SPRING  at qpos_spring: tendon_lengthspring entries that are (-1, -1) (set_const_spring; nothing without tendons);
+ * all three is set_const.  Entry i of a derived field with a leading (batch) size nb is computed from world i, for i < nb (unbatched: world
+ * 0); an output with nb > nworld is an error.  stat.meaninertia stays a Model scalar: world 0's value is written to the device array bound
+ * as "meaninertia" (mjb_model_set_array), and the caller hands it to mjb_model_set_float once it has read it back.  "actuator_acc0" is
+ * bound by name like the other arrays (batched like a float field).  d.qpos is restored bit-exactly; with restore, the position stages
+ * and the factor of M are recomputed at it for every world, otherwise the worlds that were evaluated keep the state at qpos0 / qpos_spring.
+ * Stream-ordered, no allocation, no synchronisation; the number of kernels depends on parts and restore only. */
+#define MJB_SET_CONST_FIXED 1
+#define MJB_SET_CONST_0 2
+#define MJB_SET_CONST_SPRING 4
+int mjb_set_const(const mjbModel* m, mjbData* d, int parts, int restore, void* stream);
 /* ctrl <- OU noise around ctrl_center (device array of nu floats, or NULL), reference cli.py:103-145 */
 int mjb_ctrl_noise(const mjbModel* m, mjbData* d, const float* ctrl_center, int step, float noise_std, float noise_rate, void* stream);
 

@@ -1,7 +1,8 @@
 """mujoco_warp_b200 -- H100-native (sm_90a) batched MuJoCo physics step behind the mujoco_warp API.
 
 Public surface mirrors /root/reference/mujoco_warp/__init__.py for the step path: put_model, put_data, make_data,
-reset_data, step, forward, the individually callable stages, inverse dynamics (inverse) and ray casting (ray / rays); `mjcf.load` stands in for mujoco's MJCF compiler.
+reset_data, step, forward, the individually callable stages, inverse dynamics (inverse), ray casting (ray / rays) and the
+per-world recomputation of derived Model constants (set_const, set_const_fixed, set_const_0, set_const_spring); `mjcf.load` stands in for mujoco's MJCF compiler.
 """
 
 from . import scenes
@@ -12,6 +13,7 @@ from ._src.forward import fwd_position, fwd_velocity, kinematics, last_launch_co
 from ._src.forward import com_vel, contact_force, fwd_kinematics, get_state, implicit, mul_m, passive, rne, rungekutta4, sensor_acc, sensor_pos, sensor_vel, set_state, solve_m, step1, step2
 from ._src.inverse import inverse
 from ._src.ray import ray, rays
+from ._src.set_const import set_const, set_const_0, set_const_fixed, set_const_spring
 from ._src.io import get_data_into, load_trajectory, make_data, override_model, put_data, put_model, reset_data, reset_data_keyframe
 from ._src.trace import event_trace_step, flatten_trace
 from ._src.types import BroadphaseFilter, BroadphaseType, ConeType, Constraint, ConstraintState, ConstraintType, Contact, Data

@@ -42,7 +42,7 @@ _TENDON_FLOATS = (("tendon_range", 2), ("tendon_margin", 1), ("tendon_stiffness"
                   ("tendon_length0", 1), ("tendon_invweight0", 1), ("tendon_solref_lim", 2), ("tendon_solimp_lim", 5), ("tendon_solref_fri", 2), ("tendon_solimp_fri", 5), ("tendon_actfrcrange", 2))
 # float fields outside _FLOAT_FIELDS that carry the reference's `*` leading dimension as well
 _BATCHABLE_EXTRA = ("eq_solref", "eq_solimp", "eq_data", "pair_friction", "pair_solref", "pair_solreffriction", "pair_solimp", "pair_margin", "pair_gap",
-                    "actuator_dynprm", "actuator_actrange", "geom_rgba", "mat_rgba") + tuple(n for n, _ in _TENDON_FLOATS)
+                    "actuator_dynprm", "actuator_actrange", "geom_rgba", "mat_rgba", "actuator_acc0") + tuple(n for n, _ in _TENDON_FLOATS)
 _SIZES = ["nq", "nv", "nu", "na", "nbody", "njnt", "ngeom", "nsite", "ncam", "nlight", "ntree", "nkey", "nmocap", "neq", "ntendon", "nflex"]
 
 _SUPPORTED_PAIRS = {
@@ -480,6 +480,8 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   m.actuator_actlimited = dev_i(np.asarray(getattr(mjm, "actuator_actlimited", np.zeros(nu_))).astype(np.int32))
   m.actuator_actearly = dev_i(np.asarray(getattr(mjm, "actuator_actearly", np.zeros(nu_))).astype(np.int32))
   m.actuator_dynprm = dev_f(np.asarray(getattr(mjm, "actuator_dynprm", np.zeros((nu_, 10)))).reshape(nu_, 10), name="actuator_dynprm")
+  # acceleration of a unit actuator force at qpos0 (set_const.py:493-504); nothing in the step reads it (no muscles here)
+  m.actuator_acc0 = dev_f(np.asarray(getattr(mjm, "actuator_acc0", np.zeros(nu_))).reshape(nu_), name="actuator_acc0")
   m.actuator_actrange = dev_f(np.asarray(getattr(mjm, "actuator_actrange", np.zeros((nu_, 2)))).reshape(nu_, 2), name="actuator_actrange")
   # fixed tendons (smooth.py:3658; constraint.py:642, 1867, 2243; passive.py:208): path, Jacobian sparsity and constant entries
   nt = int(getattr(mjm, "ntendon", 0))
@@ -624,7 +626,7 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
     _lib.check(L.mjb_model_set_float(h, k.encode(), float(v)))
   dev_names = {
     "jnt_limited_adr": m.jnt_limited_slide_hinge_adr, "nxn_geom_pair": m.nxn_geom_pair_filtered, "nxn_pairid": m.nxn_pairid_filtered,
-    "body_isdofancestor": m._isdofancestor_nv,
+    "body_isdofancestor": m._isdofancestor_nv, "meaninertia": m.stat.meaninertia,  # set_const writes world 0's meaninertia here
   }
   for n in (_FLOAT_FIELDS + _INT_FIELDS + ["body_childadr", "body_childid", "level_adr", "level_body", "M_entry_row", "mulm_rowadr", "mulm_col",
                                          "mulm_madr", "tree_qLDadr", "dof_fricloss_adr", "moment_rownnz0", "moment_rowadr0", "moment_colind0",
@@ -638,7 +640,7 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
                                          "ten_J_rownnz", "ten_J_rowadr", "ten_J_colind", "tendon_adr", "tendon_num", "wrap_objid", "tendon_limited", "tendon_actfrclimited", "wrap_prm", "ten_J0",
                                          "geom_group", "geom_matid", "geom_rgba", "mat_rgba", "mesh_faceadr", "mesh_face",
                                          "geom_fluid", "body_fluid", "body_geomadr", "body_geomnum", "sensor_collision_start_adr", "sensor_collision_pair",
-                                         "sensor_collision_id", "sensor_collision_adr", "sensor_collision_flip"]
+                                         "sensor_collision_id", "sensor_collision_adr", "sensor_collision_flip", "actuator_acc0"]
                                         + [n for n, _ in _TENDON_FLOATS]):
     dev_names.setdefault(n, getattr(m, n))
   for n, x in dev_names.items():
@@ -649,7 +651,7 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   _lib.check(L.mjb_model_finalize(h))
   m._keep = keep
   weakref.finalize(m, L.mjb_model_destroy, h)
-  _install_model_rebind(m, L, set(dev_names) - {"jnt_limited_adr", "nxn_geom_pair", "nxn_pairid", "body_isdofancestor"}, set(ints))
+  _install_model_rebind(m, L, set(dev_names) - {"jnt_limited_adr", "nxn_geom_pair", "nxn_pairid", "body_isdofancestor", "meaninertia"}, set(ints))
   return m
 
 
@@ -713,6 +715,12 @@ def _install_model_rebind(m: types.Model, L, arrays, ints):
     if name == "meaninertia":
       v = float(value.reshape(-1)[0]) if isinstance(value, torch.Tensor) else float(value)
       _lib.check(L.mjb_model_set_float(h, b"meaninertia", v))
+      old = m.stat.__dict__.get("meaninertia")
+      if (isinstance(value, torch.Tensor) and value.numel() >= 1 and value.device.type != "cpu" and value.dtype == torch.float32
+          and (not isinstance(old, torch.Tensor) or value.data_ptr() != old.data_ptr())):
+        x = _ptr_tensor(value.contiguous())
+        m._keep.append(x)
+        _lib.check(L.mjb_model_set_array(h, b"meaninertia", x.data_ptr(), 1))  # set_const's output follows the Statistic's tensor
     return value
 
   object.__setattr__(m, "_rebind", model_hook)

@@ -14,6 +14,7 @@ struct mjbModel {
   ModelDev dev;
   FluidDev fluid;  // qfrc_fluid stays null here: it is the Data's (fluid() below)
   SensorCollisionDev sc;
+  SetConstDev setc;  // actuator_acc0 and the meaninertia output, bound by name; qpos_save stays null here (the Data's)
   bool finalized;
 };
 struct mjbData {
@@ -29,6 +30,7 @@ struct mjbData {
   float* qfrc_inverse;  // Data.qfrc_inverse, (nworld, nv), bound by name like the DataDev arrays
   float* inv_qacc;      // (nworld, nv) continuous-time acceleration of discrete inverse dynamics, read by its sensor launch
   float* qfrc_fluid;    // Data.qfrc_fluid, (nworld, nv), bound by name; passed to the fluid kernels in FluidDev
+  float* qpos_save;     // (nworld, nq) d.qpos while mjb_set_const runs the position stages at qpos0 / qpos_spring
 };
 
 namespace {
@@ -55,6 +57,7 @@ mjbModel* mjb_model_create(void) {
   memset(&m->dev, 0, sizeof(ModelDev));
   memset(&m->fluid, 0, sizeof(FluidDev));
   memset(&m->sc, 0, sizeof(SensorCollisionDev));
+  memset(&m->setc, 0, sizeof(SetConstDev));
   m->finalized = false;
   return m;
 }
@@ -93,6 +96,12 @@ int mjb_model_set_array_batched(mjbModel* m, const char* name, const void* p, in
 #define X(n) if (!strcmp(name, #n)) { if (nbatch != 1) return fail(std::string("shared by all worlds (not batched): ") + name); m->sc.n = (const int*)p; return 0; }
   MJB_SENSCOL_IARRS(X)
 #undef X
+  if (!strcmp(name, "actuator_acc0")) { m->setc.actuator_acc0 = (float*)p; m->setc.nb_actuator_acc0 = nbatch; return 0; }
+  if (!strcmp(name, "meaninertia")) {
+    if (nbatch != 1) return fail("meaninertia is a Model scalar (not batched)");
+    m->setc.meaninertia = (float*)p;
+    return 0;
+  }
 #define X(n) if (!strcmp(name, #n)) { m->dev.n = (const float*)p; m->dev.nb_##n = nbatch; m->dev.bs_##n = batch_stride; goto done; }
   MJB_MODEL_FARRS(X)
 #undef X
@@ -140,6 +149,7 @@ mjbData* mjb_data_create(int nworld, int nconmax, int naconmax, int njmax, int n
   d->qfrc_inverse = nullptr;
   d->inv_qacc = nullptr;
   d->qfrc_fluid = nullptr;
+  d->qpos_save = nullptr;
   return d;
 }
 void mjb_data_destroy(mjbData* d) {
@@ -149,6 +159,7 @@ void mjb_data_destroy(mjbData* d) {
   if (d->dev.imp_qacc) cudaFree(d->dev.imp_qacc);
   if (d->inv_qacc) cudaFree(d->inv_qacc);
   if (d->rk) cudaFree(d->rk);
+  if (d->qpos_save) cudaFree(d->qpos_save);
   if (d->nsplit > 1) {
     for (int i = 0; i < d->nsplit; i++) { cudaStreamDestroy(d->aux[i]); cudaEventDestroy(d->ev_join[i]); }
     cudaEventDestroy(d->ev_fork);
@@ -187,6 +198,8 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
   if (check(cudaMalloc(&d->dev.imp_qacc, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nv > 0 ? m->dev.nv : 1)), "cudaMalloc(imp_qacc)")) return -1;
   // likewise always there, so that enabling discrete inverse dynamics (Option.enableflags) needs no allocation either
   if (!d->inv_qacc && check(cudaMalloc(&d->inv_qacc, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nv > 0 ? m->dev.nv : 1)), "cudaMalloc(inv_qacc)")) return -1;
+  // set_const's save buffer, so that mjb_set_const allocates nothing (and can be captured in a graph)
+  if (!d->qpos_save && check(cudaMalloc(&d->qpos_save, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nq > 0 ? m->dev.nq : 1)), "cudaMalloc(qpos_save)")) return -1;
   if (m->dev.integrator == INT_RK4 && !d->rk &&
       check(cudaMalloc(&d->rk, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nq + 3 * m->dev.nv + 2 * m->dev.na + 1)), "cudaMalloc(rk)")) return -1;
   const size_t smem[6] = {smem_position(m->dev, d->dev), smem_collision(m->dev, d->dev), smem_constraint(m->dev, d->dev),
@@ -406,6 +419,62 @@ int mjb_team_residency(const mjbModel* m, const mjbData* d, int* position_worlds
   if (check(resident_worlds_velocity(m->dev, d->dev, velocity_worlds, fluid(m, d)), "resident_worlds_velocity")) return -1;
   return 0;
 }
+int mjb_set_const(const mjbModel* m, mjbData* d, int parts, int restore, void* stream) {
+  MJB_ENTER();
+  if (parts < 1 || parts > (MJB_SET_CONST_FIXED | MJB_SET_CONST_0 | MJB_SET_CONST_SPRING)) return fail("mjb_set_const: parts must be a non-empty combination of MJB_SET_CONST_FIXED / _0 / _SPRING, got " + std::to_string(parts));
+  if (restore != 0 && restore != 1) return fail("mjb_set_const: restore must be 0 or 1");
+  const ModelDev& md = m->dev;
+  const int nworld = d->dev.nworld;
+  const bool fixed = parts & MJB_SET_CONST_FIXED, zero = parts & MJB_SET_CONST_0, spring = (parts & MJB_SET_CONST_SPRING) && md.ntendon > 0;
+  if (zero && (!m->setc.actuator_acc0 || !m->setc.meaninertia)) return fail("mjb_set_const: model array not set: actuator_acc0 / meaninertia");
+  // the worlds each part stores: a derived field with nb entries takes worlds [0, nb)
+  int w_zero = 1, w_spring = md.nb_tendon_lengthspring;
+  struct { const char* name; int nb; } out[] = {
+    {"body_subtreemass", fixed ? md.nb_body_subtreemass : 1}, {"tendon_lengthspring", spring ? md.nb_tendon_lengthspring : 1},
+    {"tendon_length0", md.nb_tendon_length0}, {"eq_data", md.nb_eq_data}, {"dof_invweight0", md.nb_dof_invweight0}, {"body_invweight0", md.nb_body_invweight0},
+    {"tendon_invweight0", md.nb_tendon_invweight0}, {"cam_pos0", md.nb_cam_pos0}, {"cam_poscom0", md.nb_cam_poscom0}, {"cam_mat0", md.nb_cam_mat0},
+    {"light_pos0", md.nb_light_pos0}, {"light_poscom0", md.nb_light_poscom0}, {"light_dir0", md.nb_light_dir0}, {"actuator_acc0", m->setc.nb_actuator_acc0},
+    {"actuator_biasprm", md.nb_actuator_biasprm}};
+  for (size_t i = 0; i < sizeof(out) / sizeof(out[0]); i++) {
+    const int nb = (i < 2 || zero) ? out[i].nb : 1;
+    if (nb > nworld) return fail(std::string("mjb_set_const: Model.") + out[i].name + " has " + std::to_string(nb) + " entries, more than the Data's " + std::to_string(nworld) + " worlds");
+    if (i >= 2) w_zero = std::max(w_zero, nb);
+  }
+  if (zero && smem_set_const(md) > kMaxSmem) {
+    char buf[200];
+    snprintf(buf, sizeof buf, "mjb_set_const: the factor and 64 right-hand-side columns of one world need %zu B of shared memory (> %zu)", smem_set_const(md), kMaxSmem);
+    return fail(buf);
+  }
+  SetConstDev c = m->setc;
+  c.qpos_save = d->qpos_save;
+  if (fixed) MJB_LAUNCH(launch_set_const_fixed(md, md.nb_body_subtreemass, nworld, s));
+  const int nw = std::max(zero ? w_zero : 0, spring ? w_spring : 0);  // worlds that run the position stages at qpos0 / qpos_spring
+  if (nw == 0) return 0;
+  DataDev dd = d->dev;
+  dd.w0 = 0;
+  dd.wn = nw;
+  if (zero) {
+    // set_const.py:656-668: the position stages and the factor of M at qpos0, then every right-hand side of a world in one warp
+    MJB_LAUNCH(launch_set_const_qpos(md, dd, c, QPOS_SAVE_LOAD0, nw, s));
+    MJB_LAUNCH(launch_position(md, dd, STG_KINEMATICS | STG_COM_POS | STG_CAMLIGHT | STG_CRB | STG_TRANSMISSION, s));
+    MJB_LAUNCH(launch_velocity(md, dd, STG_FACTOR_ONLY, s, fluid(m, d)));
+    MJB_LAUNCH(launch_set_const_0(md, dd, c, w_zero, s));
+  }
+  if (spring) {
+    // set_const.py:856-870: kinematics, com_pos, tendon and transmission at qpos_spring
+    MJB_LAUNCH(launch_set_const_qpos(md, dd, c, zero ? QPOS_LOADSPRING : QPOS_SAVE_LOADSPRING, nw, s));
+    MJB_LAUNCH(launch_position(md, dd, STG_KINEMATICS | STG_COM_POS | STG_TRANSMISSION, s));
+    MJB_LAUNCH(launch_set_const_spring(md, dd, w_spring, s));
+  }
+  MJB_LAUNCH(launch_set_const_qpos(md, dd, c, QPOS_RESTORE, nw, s));
+  if (restore) {
+    // set_const.py:835-844, 874-878, 940-949: the position stages and the factor of M at the restored qpos, for every world
+    MJB_LAUNCH(launch_position(md, d->dev, STG_KINEMATICS | STG_COM_POS | STG_CAMLIGHT | STG_CRB | STG_TRANSMISSION, s));
+    MJB_LAUNCH(launch_velocity(md, d->dev, STG_FACTOR_ONLY, s, fluid(m, d)));
+  }
+  return 0;
+}
+
 int mjb_ctrl_noise(const mjbModel* m, mjbData* d, const float* ctrl_center, int step, float noise_std, float noise_rate, void* stream) {
   MJB_ENTER();
   MJB_LAUNCH(launch_ctrl_noise(m->dev, d->dev, ctrl_center, step, noise_std, noise_rate, s));

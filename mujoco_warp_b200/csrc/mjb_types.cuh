@@ -147,6 +147,17 @@ struct SensorCollisionDev {
   const int* __restrict__ sensor_collision_flip;       // (like start_adr) the entry's geom1 is the narrowphase's second geom
 };
 
+// ---------------------------------------------------------------- set_const (k_set_const.cu)
+// The fields of mjb_set_const that are neither in ModelDev nor in DataDev, passed as one extra argument to its kernels only, for the
+// same reason as FluidDev.  Writes to the other derived Model fields go through ModelDev's pointers and nb_* / bs_*.
+struct SetConstDev {
+  float* __restrict__ actuator_acc0;  // Model.actuator_acc0 (nb_actuator_acc0, nu)
+  int nb_actuator_acc0;
+  float* __restrict__ meaninertia;    // Model.stat.meaninertia on the device (1): world 0's value
+  float* __restrict__ qpos_save;      // (nworld, nq) d.qpos while qpos0 / qpos_spring stand in for it (mjb_data_finalize allocates it)
+};
+enum { QPOS_SAVE_LOAD0 = 0, QPOS_SAVE_LOADSPRING = 1, QPOS_LOADSPRING = 2, QPOS_RESTORE = 3 };  // k_set_const_qpos modes
+
 // ---------------------------------------------------------------- enums (MuJoCo values; see constants.py)
 enum { JNT_FREE = 0, JNT_BALL = 1, JNT_SLIDE = 2, JNT_HINGE = 3 };
 enum { GEOM_PLANE = 0, GEOM_HFIELD, GEOM_SPHERE, GEOM_CAPSULE, GEOM_ELLIPSOID, GEOM_CYLINDER, GEOM_BOX, GEOM_MESH };
@@ -225,4 +236,11 @@ size_t smem_velocity(const ModelDev& m, const DataDev& d, const FluidDev& f);
 cudaError_t resident_worlds_position(const ModelDev& m, const DataDev& d, int* worlds);
 cudaError_t resident_worlds_velocity(const ModelDev& m, const DataDev& d, int* worlds, const FluidDev& f);
 size_t smem_solver(const ModelDev& m, const DataDev& d);
+// set_const (k_set_const.cu): body_subtreemass of worlds [0, nw); qpos swap of worlds [0, nw); set_const_0's outputs of worlds [0, nw)
+// from the position stages and factor at their qpos0; tendon_lengthspring of worlds [0, nw)
+cudaError_t launch_set_const_fixed(const ModelDev& m, int nw, int nworld, cudaStream_t s);
+cudaError_t launch_set_const_qpos(const ModelDev& m, const DataDev& d, const SetConstDev& c, int mode, int nw, cudaStream_t s);
+cudaError_t launch_set_const_0(const ModelDev& m, const DataDev& d, const SetConstDev& c, int nw, cudaStream_t s);
+cudaError_t launch_set_const_spring(const ModelDev& m, const DataDev& d, int nw, cudaStream_t s);
+size_t smem_set_const(const ModelDev& m);
 size_t smem_integrate(const ModelDev& m);
