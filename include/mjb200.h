@@ -27,6 +27,7 @@
  *   mjb_solve_m                <- _src/smooth.py:3214  solve_m(m, d, x, y): x = M^-1 y through Data.qLD
  *   mjb_mul_m                  <- _src/support.py:153  mul_m(m, d, res, vec): res = M vec
  *   mjb_sensor_pos/vel/acc     <- _src/sensor.py:810, :1432, :2512  sensor_pos / sensor_vel / sensor_acc(m, d)
+ *   mjb_energy_pos/vel         <- _src/sensor.py:2934, :3004  energy_pos / energy_vel(m, d)
  *   mjb_contact_force          <- _src/support.py:445  contact_force(m, d, contact_ids, to_world_frame, force)
  *   mjb_rays                   <- _src/ray.py:1219 rays(m, d, pnt, vec, geomgroup, flg_static, bodyexclude, dist, geomid, normal) without a
  *                                 render context (every geom tested, no BVH; no height fields)
@@ -108,6 +109,12 @@ int mjb_mul_m(const mjbModel* m, mjbData* d, float* res, const float* vec, void*
 int mjb_sensor_pos(const mjbModel* m, mjbData* d, void* stream);
 int mjb_sensor_vel(const mjbModel* m, mjbData* d, void* stream);
 int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream);
+/* sensor.py:2934 energy_pos / :3004 energy_vel: Data.energy[:, 0] = potential energy (gravity unless DSBL_GRAVITY; joint and fixed-tendon
+ * springs unless DSBL_SPRING) at the last position stage; Data.energy[:, 1] = 1/2 qvel . M qvel with the M of the last crb.  Whatever
+ * ENBL_ENERGY says; one kernel launch each.  Data.energy is bound by name ("energy", (nworld, 2) fp32).  forward / step / step1 compute
+ * both terms when ENBL_ENERGY is set; the e_potential / e_kinetic sensors are written by mjb_sensor_pos, forward, step and inverse. */
+int mjb_energy_pos(const mjbModel* m, mjbData* d, void* stream);
+int mjb_energy_vel(const mjbModel* m, mjbData* d, void* stream);
 /* support.py:445 contact_force(m, d, contact_ids, to_world_frame, force): force is (n, 6) floats, device pointers */
 int mjb_contact_force(const mjbModel* m, mjbData* d, const int* contact_ids, int n, int to_world_frame, float* force, void* stream);
 /* ray.py:1219 rays: pnt, vec (pnt_nbatch, nray, 3) fp32 device, pnt_nbatch 1 or nworld; geomgroup: 6 host ints (all -1 = no group

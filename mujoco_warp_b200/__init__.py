@@ -1,8 +1,8 @@
 """mujoco_warp_b200 -- H100-native (sm_90a) batched MuJoCo physics step behind the mujoco_warp API.
 
 Public surface mirrors /root/reference/mujoco_warp/__init__.py for the step path: put_model, put_data, make_data,
-reset_data, step, forward, the individually callable stages, inverse dynamics (inverse), ray casting (ray / rays) and the
-per-world recomputation of derived Model constants (set_const, set_const_fixed, set_const_0, set_const_spring); `mjcf.load` stands in for mujoco's MJCF compiler.
+reset_data, step, forward, the individually callable stages, potential and kinetic energy (energy_pos / energy_vel), inverse
+dynamics (inverse), ray casting (ray / rays) and the per-world recomputation of derived Model constants (set_const, set_const_fixed, set_const_0, set_const_spring); `mjcf.load` stands in for mujoco's MJCF compiler.
 """
 
 from . import scenes
@@ -10,6 +10,7 @@ from ._src import mjcf
 from ._src._lib import build
 from ._src.forward import camlight, collision, com_pos, crb, ctrl_noise, euler, factor_m, forward, fwd_acceleration, fwd_actuation
 from ._src.forward import fwd_position, fwd_velocity, kinematics, last_launch_count, make_constraint, solve, step, step_profile, team_residency, transmission
+from ._src.forward import energy_pos, energy_vel
 from ._src.forward import com_vel, contact_force, fwd_kinematics, get_state, implicit, mul_m, passive, rne, rungekutta4, sensor_acc, sensor_pos, sensor_vel, set_state, solve_m, step1, step2
 from ._src.inverse import inverse
 from ._src.ray import ray, rays

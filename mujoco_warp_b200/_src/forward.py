@@ -104,6 +104,20 @@ def sensor_acc(m: Model, d: Data):
   _call("mjb_sensor_acc", m, d)
 
 
+def energy_pos(m: Model, d: Data):
+  """Potential energy into d.energy[:, 0] (reference sensor.py:2934): -sum_b body_mass[b] gravity . xipos[b] unless gravity is
+  disabled, plus 1/2 k x^2 of every joint spring (hinge / slide: q - qpos_spring; ball / free: the rotation from qpos_spring, and the
+  free joint's translation) and fixed-tendon spring (x: the length outside the springlength dead band) unless springs are disabled.
+  Reads the last position stage; runs whatever `EnableBit.ENERGY` says."""
+  _call("mjb_energy_pos", m, d)
+
+
+def energy_vel(m: Model, d: Data):
+  """Kinetic energy 1/2 qvel . (M qvel) into d.energy[:, 1] (reference sensor.py:3004), with the M (armature included) of the last crb.
+  Runs whatever `EnableBit.ENERGY` says."""
+  _call("mjb_energy_vel", m, d)
+
+
 def rungekutta4(m: Model, d: Data):
   """Runge-Kutta 4 integrator, to be called after forward() (reference forward.py:523); the model must use the RK4 integrator."""
   from . import constants as C
@@ -226,14 +240,24 @@ def set_state(m: Model, d: Data, state: torch.Tensor, sig: int, active: torch.Te
 
 def step1(m: Model, d: Data):
   """First half of a split step, before the user sets controls (reference forward.py:1384 step1: position and velocity stages
-  with their sensors; energy is not computed in this build)."""
+  with their sensors, and energy).  With `EnableBit.ENERGY` set d.energy gets both terms; without it a model with e_potential /
+  e_kinetic sensors ends with d.energy zeroed, as the reference leaves it, and any other model leaves d.energy untouched."""
+  from . import constants as C
+
   fwd_position(m, d)
   if getattr(m, "nsensor", 0):
     d.sensordata.zero_()
     sensor_pos(m, d)
+  energy_on = bool(m.opt.enableflags & C.ENBL_ENERGY)
+  if energy_on:
+    energy_pos(m, d)
+  elif len(m.sensor_energy_adr):
+    d.energy.zero_()
   fwd_velocity(m, d)
   if getattr(m, "nsensor", 0):
     sensor_vel(m, d)
+  if energy_on:
+    energy_vel(m, d)
 
 
 def step2(m: Model, d: Data):

@@ -278,6 +278,11 @@ def derive_tables(mjm) -> dict:
     nmaxcondim = max(nmaxcondim, int(np.asarray(mjm.pair_dim).max()))
   t["nmaxcondim"] = nmaxcondim
   t["nmaxpyramid"] = max(1, 2 * (nmaxcondim - 1))
+  # energy sensors (reference io.py:893-894): k_energy writes their slots, k_sensor skips them
+  stype = np.asarray(mjm.sensor_type).reshape(-1) if int(getattr(mjm, "nsensor", 0)) else np.zeros(0, dtype=int)
+  t["sensor_energy_adr"] = np.nonzero(np.isin(stype, (C.SENS_E_POTENTIAL, C.SENS_E_KINETIC)))[0].astype(np.int32)
+  t["sensor_e_potential"] = bool((stype == C.SENS_E_POTENTIAL).any())
+  t["sensor_e_kinetic"] = bool((stype == C.SENS_E_KINETIC).any())
   return t
 
 
@@ -354,10 +359,10 @@ def _validate(mjm):
     raise NotImplementedError("fluid forces (opt.density / viscosity / wind) with the implicit integrator are not implemented (use implicitfast, Euler or RK4)")
   if int(getattr(o, "noslip_iterations", 0)) > 0:
     raise NotImplementedError("the noslip solver (opt.noslip_iterations > 0) is not implemented")
-  unsupported_enable = int(o.enableflags) & (C.ENBL_OVERRIDE | C.ENBL_ENERGY | C.ENBL_FWDINV | C.ENBL_SLEEP)
+  unsupported_enable = int(o.enableflags) & (C.ENBL_OVERRIDE | C.ENBL_FWDINV | C.ENBL_SLEEP)
   if unsupported_enable:
     names = [n for n, b in C.ENABLE_FLAGS.items() if unsupported_enable & b]
-    raise NotImplementedError(f"enable flag(s) {names} are not implemented (contact override, energy, fwdinv, sleeping)")
+    raise NotImplementedError(f"enable flag(s) {names} are not implemented (contact override, fwdinv, sleeping)")
   if getattr(mjm, "nu", 0):
     gt, bt = np.asarray(mjm.actuator_gaintype), np.asarray(mjm.actuator_biastype)
     if not np.isin(gt, (C.GAIN_FIXED, C.GAIN_AFFINE)).all():
@@ -538,6 +543,8 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   m.nsensorcollision, m.sensor_collision_epa_iterations, m.nsensorcollision_ccd = (sc.pop(k) for k in ("nsensorcollision", "sensor_collision_epa_iterations", "nsensorcollision_ccd"))
   for n, x in sc.items():
     setattr(m, n, dev_i(x))
+  m.sensor_energy_adr = dev_i(t["sensor_energy_adr"])
+  m.sensor_e_potential, m.sensor_e_kinetic = t["sensor_e_potential"], t["sensor_e_kinetic"]
   m.eq_type = dev_i(mjm.eq_type if neq else np.zeros(0))
   m.eq_obj1id = dev_i(mjm.eq_obj1id if neq else np.zeros(0))
   m.eq_obj2id = dev_i(mjm.eq_obj2id if neq else np.zeros(0))
@@ -615,7 +622,8 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   for k, v in ints.items():
     _lib.check(L.mjb_model_set_int(h, k.encode(), int(v)))
   for k, v in (("nsensorcollision", m.nsensorcollision), ("nsensorcollision_sensor", len(m.sensor_collision_id)), ("sensor_collision_epa_iterations", m.sensor_collision_epa_iterations),
-               ("nsensorcollision_ccd", m.nsensorcollision_ccd)):
+               ("nsensorcollision_ccd", m.nsensorcollision_ccd), ("nsensor_energy", len(t["sensor_energy_adr"])),
+               ("sensor_e_potential", m.sensor_e_potential), ("sensor_e_kinetic", m.sensor_e_kinetic)):
     _lib.check(L.mjb_model_set_int(h, k.encode(), int(v)))
   g = np.asarray(o.gravity, dtype=np.float64)
   floats = dict(timestep=o.timestep, tolerance=tol, ls_tolerance=o.ls_tolerance, impratio_invsqrt=1.0 / np.sqrt(o.impratio),
@@ -640,7 +648,7 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
                                          "ten_J_rownnz", "ten_J_rowadr", "ten_J_colind", "tendon_adr", "tendon_num", "wrap_objid", "tendon_limited", "tendon_actfrclimited", "wrap_prm", "ten_J0",
                                          "geom_group", "geom_matid", "geom_rgba", "mat_rgba", "mesh_faceadr", "mesh_face",
                                          "geom_fluid", "body_fluid", "body_geomadr", "body_geomnum", "sensor_collision_start_adr", "sensor_collision_pair",
-                                         "sensor_collision_id", "sensor_collision_adr", "sensor_collision_flip", "actuator_acc0"]
+                                         "sensor_collision_id", "sensor_collision_adr", "sensor_collision_flip", "actuator_acc0", "sensor_energy_adr"]
                                         + [n for n, _ in _TENDON_FLOATS]):
     dev_names.setdefault(n, getattr(m, n))
   for n, x in dev_names.items():
@@ -791,7 +799,7 @@ _BOUND_TOP = [
   "crb", "M", "qLD", "actuator_length", "actuator_moment", "actuator_velocity", "cvel", "cdof_dot", "qfrc_bias", "qfrc_spring", "qfrc_damper",
   "qfrc_gravcomp", "qfrc_passive", "actuator_force", "qfrc_actuator", "qfrc_smooth", "qacc_smooth", "qfrc_constraint", "qfrc_inverse", "cacc", "cfrc_int",
   "ne", "nf", "nl", "nefc", "nacon", "ncollision", "solver_niter", "overflow", "moment_rownnz", "moment_rowadr", "moment_colind", "eq_active", "mocap_pos", "mocap_quat", "sensordata", "subtree_linvel", "subtree_angmom", "cfrc_ext",
-  "act", "act_dot", "ten_length", "ten_J", "ten_velocity", "qLU", "qfrc_fluid",
+  "act", "act_dot", "ten_length", "ten_J", "ten_velocity", "qLU", "qfrc_fluid", "energy",
 ]
 _BOUND_EFC = ["J", "pos", "margin", "D", "vel", "aref", "frictionloss", "force", "Ma", "type", "id", "state"]
 _BOUND_CONTACT = ["dist", "pos", "frame", "includemargin", "friction", "solref", "solreffriction", "solimp", "dim", "geom", "efc_address", "worldid", "type", "geomcollisionid"]

@@ -1458,6 +1458,8 @@ def compile_xml(root):
     "framelinacc": (S.SENS_FRAMELINACC, "obj", 3, 0, 3), "frameangacc": (S.SENS_FRAMEANGACC, "obj", 3, 0, 3),
     # collision sensors between two geoms or bodies: signed distance, unit normal (AXIS), and the two witness points
     "distance": (S.SENS_GEOMDIST, "pair", 1, 0, 1), "normal": (S.SENS_GEOMNORMAL, "pair", 3, 2, 1), "fromto": (S.SENS_GEOMFROMTO, "pair", 6, 0, 1),
+    # potential and kinetic energy of the whole model (no object)
+    "e_potential": (S.SENS_E_POTENTIAL, None, 1, 0, 1), "e_kinetic": (S.SENS_E_KINETIC, None, 1, 0, 1),
   }
   objkind = {"tendon": (C.OBJ_TENDON, "tendon"), "joint": (C.OBJ_JOINT, "joint"), "actuator": (C.OBJ_ACTUATOR, "actuator"), "site": (C.OBJ_SITE, "site"), "body": (C.OBJ_BODY, "body")}
   objtypes = {"body": (C.OBJ_BODY, "body"), "xbody": (C.OBJ_XBODY, "body"), "geom": (C.OBJ_GEOM, "geom"), "site": (C.OBJ_SITE, "site"), "camera": (C.OBJ_CAMERA, "camera")}

@@ -15,6 +15,7 @@ struct mjbModel {
   FluidDev fluid;  // qfrc_fluid stays null here: it is the Data's (fluid() below)
   SensorCollisionDev sc;
   SetConstDev setc;  // actuator_acc0 and the meaninertia output, bound by name; qpos_save stays null here (the Data's)
+  EnergyDev en;      // the energy sensors; energy stays null here (the Data's: energy() below)
   bool finalized;
 };
 struct mjbData {
@@ -31,6 +32,7 @@ struct mjbData {
   float* inv_qacc;      // (nworld, nv) continuous-time acceleration of discrete inverse dynamics, read by its sensor launch
   float* qfrc_fluid;    // Data.qfrc_fluid, (nworld, nv), bound by name; passed to the fluid kernels in FluidDev
   float* qpos_save;     // (nworld, nq) d.qpos while mjb_set_const runs the position stages at qpos0 / qpos_spring
+  float* energy;        // Data.energy, (nworld, 2), bound by name; passed to k_energy in EnergyDev
 };
 
 namespace {
@@ -45,6 +47,8 @@ constexpr size_t kMaxSmem = 227 * 1024;
 
 // The fluid fields of a model bound to a Data's qfrc_fluid
 static FluidDev fluid(const mjbModel* m, const mjbData* d) { FluidDev f = m->fluid; f.qfrc_fluid = d->qfrc_fluid; return f; }
+// The energy sensors of a model bound to a Data's energy
+static EnergyDev energy(const mjbModel* m, const mjbData* d) { EnergyDev e = m->en; e.energy = d->energy; return e; }
 
 extern "C" {
 
@@ -58,6 +62,7 @@ mjbModel* mjb_model_create(void) {
   memset(&m->fluid, 0, sizeof(FluidDev));
   memset(&m->sc, 0, sizeof(SensorCollisionDev));
   memset(&m->setc, 0, sizeof(SetConstDev));
+  memset(&m->en, 0, sizeof(EnergyDev));
   m->finalized = false;
   return m;
 }
@@ -72,6 +77,9 @@ int mjb_model_set_int(mjbModel* m, const char* name, int v) {
 #undef X
 #define X(n) if (!strcmp(name, #n)) { m->sc.n = v; return 0; }
   MJB_SENSCOL_INTS(X)
+#undef X
+#define X(n) if (!strcmp(name, #n)) { m->en.n = v; return 0; }
+  MJB_ENERGY_INTS(X)
 #undef X
   return fail(std::string("unknown model int field: ") + name);
 }
@@ -95,6 +103,9 @@ int mjb_model_set_array_batched(mjbModel* m, const char* name, const void* p, in
 #undef X
 #define X(n) if (!strcmp(name, #n)) { if (nbatch != 1) return fail(std::string("shared by all worlds (not batched): ") + name); m->sc.n = (const int*)p; return 0; }
   MJB_SENSCOL_IARRS(X)
+#undef X
+#define X(n) if (!strcmp(name, #n)) { if (nbatch != 1) return fail(std::string("shared by all worlds (not batched): ") + name); m->en.n = (const int*)p; return 0; }
+  MJB_ENERGY_IARRS(X)
 #undef X
   if (!strcmp(name, "actuator_acc0")) { m->setc.actuator_acc0 = (float*)p; m->setc.nb_actuator_acc0 = nbatch; return 0; }
   if (!strcmp(name, "meaninertia")) {
@@ -129,6 +140,9 @@ int mjb_model_finalize(mjbModel* m) {
 #define X(n) if (!m->sc.n) return fail(std::string("model array not set: ") + #n);
   MJB_SENSCOL_IARRS(X)
 #undef X
+#define X(n) if (!m->en.n) return fail(std::string("model array not set: ") + #n);
+  MJB_ENERGY_IARRS(X)
+#undef X
   if (m->dev.nv <= 0 || m->dev.nbody <= 0) return fail("model has no dofs/bodies");
   if (m->dev.solver != SOL_NEWTON && m->dev.solver != SOL_CG) return fail("only the Newton and CG solvers are implemented");
   if (m->dev.cone != CONE_PYRAMIDAL && m->dev.cone != CONE_ELLIPTIC) return fail("unknown friction cone type");
@@ -150,6 +164,7 @@ mjbData* mjb_data_create(int nworld, int nconmax, int naconmax, int njmax, int n
   d->inv_qacc = nullptr;
   d->qfrc_fluid = nullptr;
   d->qpos_save = nullptr;
+  d->energy = nullptr;
   return d;
 }
 void mjb_data_destroy(mjbData* d) {
@@ -173,6 +188,7 @@ int mjb_data_set_int(mjbData* d, const char* name, int v) {
 int mjb_data_set_array(mjbData* d, const char* name, void* p) {
   if (!strcmp(name, "qfrc_inverse")) { d->qfrc_inverse = (float*)p; return 0; }
   if (!strcmp(name, "qfrc_fluid")) { d->qfrc_fluid = (float*)p; return 0; }
+  if (!strcmp(name, "energy")) { d->energy = (float*)p; return 0; }
 #define X(n) if (!strcmp(name, #n)) { d->dev.n = (float*)p; return 0; }
   MJB_DATA_FARRS(X)
 #undef X
@@ -189,6 +205,7 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
 #undef X
   if (!d->qfrc_inverse) return fail("data array not set: qfrc_inverse");
   if (!d->qfrc_fluid) return fail("data array not set: qfrc_fluid");
+  if (!d->energy) return fail("data array not set: energy");
   if (d->dev.nv_pad < m->dev.nv) return fail("nv_pad < nv");
   if (check(cudaMalloc(&d->dev.world_conadr, sizeof(int) * (size_t)d->dev.nworld), "cudaMalloc(world_conadr)")) return -1;
   if (check(cudaMalloc(&d->dev.world_ncon, sizeof(int) * (size_t)d->dev.nworld), "cudaMalloc(world_ncon)")) return -1;
@@ -288,7 +305,28 @@ int mjb_rays(const mjbModel* m, mjbData* d, const float* pnt, const float* vec, 
   MJB_LAUNCH(launch_ray(m->dev, d->dev, pnt, vec, nray, pnt_nbatch, geomgroup, flg_static, bodyexclude, dist, geomid, normal, s));
   return 0;
 }
-int mjb_sensor_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 1, s, m->sc)); return 0; }
+// The k_energy parts of the position-stage sensors (sensor.py:845-849): the terms the energy sensors read, and the sensors themselves
+static int energy_sensor_parts(const mjbModel* m) {
+  if (m->en.nsensor_energy == 0 || (m->dev.disableflags & DSBL_SENSOR)) return 0;
+  return ENERGY_SENSOR | (m->en.sensor_e_potential ? ENERGY_POT : 0) | (m->en.sensor_e_kinetic ? ENERGY_KIN : 0);
+}
+// The k_energy parts of forward (forward.py:1327-1356): with ENBL_ENERGY both terms, and the energy sensors unless DSBL_SENSOR is set (the
+// reference then leaves Data.energy stale; here it is computed); without it the sensors' terms, after which Data.energy is zeroed as the
+// reference does.  0 (no launch, Data.energy untouched) for a model with the flag off and no energy sensor.
+static int energy_forward_parts(const mjbModel* m) {
+  const int sens = energy_sensor_parts(m);
+  if (m->dev.enableflags & ENBL_ENERGY) return ENERGY_POT | ENERGY_KIN | sens;
+  return m->en.nsensor_energy > 0 ? sens | ENERGY_ZERO : 0;
+}
+
+int mjb_sensor_pos(const mjbModel* m, mjbData* d, void* stream) {
+  MJB_ENTER();
+  MJB_LAUNCH(launch_sensor(m->dev, d->dev, 1, s, m->sc));
+  MJB_LAUNCH(launch_energy(m->dev, d->dev, energy(m, d), energy_sensor_parts(m), s));
+  return 0;
+}
+int mjb_energy_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_energy(m->dev, d->dev, energy(m, d), ENERGY_POT, s)); return 0; }
+int mjb_energy_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_energy(m->dev, d->dev, energy(m, d), ENERGY_KIN, s)); return 0; }
 int mjb_sensor_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 2, s, m->sc)); return 0; }
 int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 4, s, m->sc)); return 0; }
 int mjb_solve(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_solver(m->dev, d->dev, s)); return 0; }
@@ -326,6 +364,8 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
     MJB_LAUNCH(launch_solver(m->dev, dd, s));
     // sensors of all three stages in one launch after the solver (forward.py:1350-1365 interleaves them; their inputs are final by now)
     if (m->dev.nsensor > 0) MJB_LAUNCH(launch_sensor(m->dev, dd, 7, s, m->sc));
+    // energy after the sensors (the reference's energy_pos / energy_vel, forward.py:1327-1356): its inputs are final since fwd_velocity
+    MJB_LAUNCH(launch_energy(m->dev, dd, energy(m, d), energy_forward_parts(m), s));
     MJB_MARK(4);
   }
   if (what & RUN_INVERSE) {
@@ -338,6 +378,7 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
       if (disc) ds.qacc = d->inv_qacc;
       MJB_LAUNCH(launch_sensor(m->dev, ds, 7, s, m->sc));
     }
+    MJB_LAUNCH(launch_energy(m->dev, dd, energy(m, d), energy_sensor_parts(m), s));  // inverse computes energy only for its sensors
   }
   if (what & RUN_EULER) {
     if (m->dev.integrator == INT_IMPLICIT && smem_implicit(m->dev) > kMaxSmem) return fail("implicit integrator: the velocity-derivative scratch (18 x nbody x 32 floats) exceeds one block's shared memory");

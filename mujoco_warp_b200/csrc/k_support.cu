@@ -121,11 +121,7 @@ k_mul_m(const __grid_constant__ ModelDev m, const __grid_constant__ DataDev d, f
   __syncwarp();
   const float* M = d.M + wb * m.nC;
 #pragma unroll 1
-  for (int i = lane; i < m.nv; i += 32) {
-    float acc = 0.f;
-    for (int k = m.mulm_rowadr[i]; k < m.mulm_rowadr[i + 1]; k++) acc += M[m.mulm_madr[k]] * v[m.mulm_col[k]];
-    res[wb * m.nv + i] = acc;
-  }
+  for (int i = lane; i < m.nv; i += 32) res[wb * m.nv + i] = mul_m_row(m, M, v, i);
 }
 
 // support.py:326-442 contact_force: 6D force / torque of the listed contacts, in the contact frame unless to_world is set

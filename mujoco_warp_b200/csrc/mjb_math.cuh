@@ -112,6 +112,12 @@ __device__ __forceinline__ float tendon_J_at(const ModelDev& m, int t, int c) {
   for (int k = 0; k < n; k++) if (m.ten_J_colind[adr + k] == c) return m.ten_J0[adr + k];
   return 0.f;
 }
+// support.py:153-256 mul_m: row i of M v for one world's M (nC entries) through the symmetric gather tables; v in shared memory
+__device__ __forceinline__ float mul_m_row(const ModelDev& m, const float* M, const float* v, int i) {
+  float acc = 0.f;
+  for (int k = m.mulm_rowadr[i]; k < m.mulm_rowadr[i + 1]; k++) acc += M[m.mulm_madr[k]] * v[m.mulm_col[k]];
+  return acc;
+}
 // support.py:38-64 next_act: one integration step of actuator a's activation (exact for FILTEREXACT), optionally clamped to actrange
 __device__ __forceinline__ float next_act(const ModelDev& m, int a, float act, float act_dot, float scale, bool clamp) {
   float r;

@@ -158,6 +158,20 @@ struct SetConstDev {
 };
 enum { QPOS_SAVE_LOAD0 = 0, QPOS_SAVE_LOADSPRING = 1, QPOS_LOADSPRING = 2, QPOS_RESTORE = 3 };  // k_set_const_qpos modes
 
+// ---------------------------------------------------------------- energy (k_energy.cu)
+// Data.energy and the e_potential / e_kinetic sensors, passed as one extra argument to k_energy only, for the same reason as FluidDev.
+#define MJB_ENERGY_INTS(X) X(nsensor_energy) X(sensor_e_potential) X(sensor_e_kinetic)
+#define MJB_ENERGY_IARRS(X) X(sensor_energy_adr)
+struct EnergyDev {
+  int nsensor_energy;                         // e_potential and e_kinetic sensors
+  int sensor_e_potential, sensor_e_kinetic;   // the model has a sensor of that type
+  const int* __restrict__ sensor_energy_adr;  // (nsensor_energy) their sensor ids
+  float* __restrict__ energy;                 // Data.energy (nworld, 2): potential, kinetic
+};
+// k_energy parts: the potential and kinetic terms into Data.energy, the energy sensors from them, and Data.energy zeroed afterwards
+// (forward with ENBL_ENERGY off: the sensors report, Data.energy ends at zero)
+enum { ENERGY_POT = 1, ENERGY_KIN = 2, ENERGY_SENSOR = 4, ENERGY_ZERO = 8 };
+
 // ---------------------------------------------------------------- enums (MuJoCo values; see constants.py)
 enum { JNT_FREE = 0, JNT_BALL = 1, JNT_SLIDE = 2, JNT_HINGE = 3 };
 enum { GEOM_PLANE = 0, GEOM_HFIELD, GEOM_SPHERE, GEOM_CAPSULE, GEOM_ELLIPSOID, GEOM_CYLINDER, GEOM_BOX, GEOM_MESH };
@@ -171,7 +185,7 @@ enum { OBJ_BODY = 1, OBJ_XBODY = 2, OBJ_GEOM = 5, OBJ_SITE = 6, OBJ_CAMERA = 7 }
 enum { SENS_TOUCH = 0, SENS_ACCELEROMETER = 1, SENS_VELOCIMETER = 2, SENS_GYRO = 3, SENS_FORCE = 4, SENS_TORQUE = 5, SENS_JOINTPOS = 9, SENS_JOINTVEL = 10, SENS_TENDONPOS = 11, SENS_TENDONVEL = 12, SENS_ACTUATORPOS = 13, SENS_ACTUATORVEL = 14,
        SENS_ACTUATORFRC = 15, SENS_JOINTACTFRC = 16, SENS_BALLQUAT = 18, SENS_BALLANGVEL = 19, SENS_JOINTLIMITPOS = 20, SENS_JOINTLIMITVEL = 21, SENS_JOINTLIMITFRC = 22, SENS_FRAMEPOS = 26, SENS_FRAMEQUAT = 27, SENS_FRAMEXAXIS = 28,
        SENS_FRAMEYAXIS = 29, SENS_FRAMEZAXIS = 30, SENS_FRAMELINVEL = 31, SENS_FRAMEANGVEL = 32, SENS_FRAMELINACC = 33, SENS_FRAMEANGACC = 34, SENS_SUBTREECOM = 35, SENS_SUBTREELINVEL = 36, SENS_SUBTREEANGMOM = 37, SENS_GEOMDIST = 39, SENS_GEOMNORMAL = 40,
-       SENS_GEOMFROMTO = 41, SENS_CLOCK = 45 };
+       SENS_GEOMFROMTO = 41, SENS_E_POTENTIAL = 43, SENS_E_KINETIC = 44, SENS_CLOCK = 45 };
 enum { CNSTR_EQUALITY = 0, CNSTR_FRICTION_DOF = 1, CNSTR_FRICTION_TENDON = 2, CNSTR_LIMIT_JOINT = 3, CNSTR_LIMIT_TENDON = 4, CNSTR_CONTACT_FRICTIONLESS = 5, CNSTR_CONTACT_PYRAMIDAL = 6, CNSTR_CONTACT_ELLIPTIC = 7 };
 enum { ST_SATISFIED = 0, ST_QUADRATIC = 1, ST_LINEARNEG = 2, ST_LINEARPOS = 3, ST_CONE = 4 };
 enum { CAM_FIXED = 0, CAM_TRACK, CAM_TRACKCOM, CAM_TARGETBODY, CAM_TARGETBODYCOM };
@@ -183,7 +197,7 @@ enum {
   DSBL_SPRING = 1 << 5, DSBL_DAMPER = 1 << 6, DSBL_GRAVITY = 1 << 7, DSBL_CLAMPCTRL = 1 << 8, DSBL_WARMSTART = 1 << 9,
   DSBL_ACTUATION = 1 << 11, DSBL_REFSAFE = 1 << 12, DSBL_SENSOR = 1 << 13, DSBL_EULERDAMP = 1 << 15, DSBL_NATIVECCD = 1 << 17
 };
-enum { ENBL_INVDISCRETE = 1 << 3 };
+enum { ENBL_ENERGY = 1 << 1, ENBL_INVDISCRETE = 1 << 3 };
 enum { OVF_NEFC = 1 << 0, OVF_NJMAX_NNZ = 1 << 1, OVF_BROADPHASE = 1 << 2, OVF_NARROWPHASE = 1 << 3, OVF_EPA_HORIZON = 1 << 8, OVF_ITERATIONS = 1 << 9, OVF_LS_ITERATIONS = 1 << 10 };
 enum { BF_PLANE = 1, BF_SPHERE = 2, BF_AABB = 4, BF_OBB = 8 };
 enum { CONTACT_TYPE_CONSTRAINT = 1, CONTACT_TYPE_SENSOR = 2 };
@@ -243,4 +257,6 @@ cudaError_t launch_set_const_qpos(const ModelDev& m, const DataDev& d, const Set
 cudaError_t launch_set_const_0(const ModelDev& m, const DataDev& d, const SetConstDev& c, int nw, cudaStream_t s);
 cudaError_t launch_set_const_spring(const ModelDev& m, const DataDev& d, int nw, cudaStream_t s);
 size_t smem_set_const(const ModelDev& m);
+// energy (k_energy.cu): the ENERGY_* parts of d's world range
+cudaError_t launch_energy(const ModelDev& m, const DataDev& d, const EnergyDev& e, int parts, cudaStream_t s);
 size_t smem_integrate(const ModelDev& m);

@@ -363,6 +363,8 @@ class array:
       if not 0 <= i < n:
         raise IndexError(f"index {idx} out of range for shape {self.shape}")
     if len(idx) == len(self.shape):
+      if isinstance(self.dtype, type) and issubclass(self.dtype, Vec) and _component_store(sys._getframe(1)):
+        return _ComponentRef(self.a, idx)
       return self._wrap(self.a[idx])
     return array._view(self.a[idx], self.dtype)
 
@@ -445,6 +447,30 @@ def _tile_from(src, dtype):
   for i in _np.ndindex(outer):
     out[i] = dtype([dtype._conv(x) for x in src[i]]) if issubclass(dtype, Vec) else dtype._from_rows(src[i].tolist())
   return out
+
+
+class _ComponentRef:
+  """`arr[i]` as the target of a component store `arr[i][k] = v`, which in warp writes into the array (a plain read returns a copy)"""
+
+  __slots__ = ("a", "idx")
+
+  def __init__(self, a, idx):
+    self.a, self.idx = a, idx
+
+  def __setitem__(self, k, v):
+    self.a[self.idx + (int(k),)] = v
+
+
+_STORE_CACHE = {}
+
+
+def _component_store(frame):
+  """whether the instruction after the caller's subscript loads one index and stores into the element: `arr[i][k] = v`"""
+  key = (frame.f_code, frame.f_lasti)
+  if key not in _STORE_CACHE:
+    nxt = [ins.opname for ins in _dis.get_instructions(frame.f_code) if ins.offset > frame.f_lasti][:2]
+    _STORE_CACHE[key] = len(nxt) == 2 and nxt[0] in ("LOAD_CONST", "LOAD_FAST") and nxt[1] == "STORE_SUBSCR"
+  return _STORE_CACHE[key]
 
 
 _UNPACK_CACHE = {}
