@@ -155,8 +155,11 @@ int mjb_step_profile(const mjbModel* m, mjbData* d, void* stream, float* ms_out)
 
 /* worlds per SM that are resident at once (cudaOccupancyMaxActiveBlocksPerMultiprocessor times worlds per block) in the launch
  * shape k_position / k_velocity take for all of d's worlds.  Both kernels are latency bound: they finish in
- * ceil(nworld / (SMs x worlds per SM)) rounds of one world's dependent chain. */
-int mjb_team_residency(const mjbModel* m, const mjbData* d, int* position_worlds, int* velocity_worlds);
+ * ceil(nworld / (SMs x worlds per SM)) rounds of one world's dependent chain.  shapes (host pointer to 8 ints, or NULL) receives the
+ * launch shape behind each count, k_position's in shapes[0..3] and k_velocity's in shapes[4..7]: lanes per world (8, 16 or 32), warps
+ * per block, shared-memory bytes per block, and the instance (k_velocity: 0 plain, 1 with gravity compensation / ball and free joint
+ * springs / tendons, 2 with fluid forces; k_position: 0). */
+int mjb_team_residency(const mjbModel* m, const mjbData* d, int* position_worlds, int* velocity_worlds, int* shapes);
 
 /* number of kernels launched by the calling thread's last mjb_* call that enqueues work, counted at each launch (memsets are not
  * kernels and are not counted); bench.py's gpu_launches */

@@ -301,13 +301,21 @@ def step_profile(m: Model, d: Data):
   return dict(zip(KERNEL_NAMES, [float(x) for x in out]))
 
 
-def team_residency(m: Model, d: Data):
+TEAM_INSTANCES = ("plain", "pext", "fluid")
+
+
+def team_residency(m: Model, d: Data, shapes: bool = False):
   """Worlds per SM resident at once in the launch shape of k_position / k_velocity for all of d's worlds (occupancy API);
-  returns {"position": n, "velocity": n}."""
+  returns {"position": n, "velocity": n}.  With shapes=True each kernel maps to the launch shape as well:
+  {"worlds_per_sm": n, "lpw": lanes per world, "wpb": warps per block, "block_bytes": shared memory per block,
+  "instance": "plain" | "pext" | "fluid" (k_position is always "plain")}."""
   import ctypes
 
   f = _lib.lib().mjb_team_residency
-  f.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]
-  pos, vel = ctypes.c_int(), ctypes.c_int()
-  _lib.check(f(m._handle, d._handle, ctypes.byref(pos), ctypes.byref(vel)))
-  return {"position": pos.value, "velocity": vel.value}
+  f.argtypes = [ctypes.c_void_p, ctypes.c_void_p, ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int), ctypes.POINTER(ctypes.c_int)]
+  pos, vel, sh = ctypes.c_int(), ctypes.c_int(), (ctypes.c_int * 8)()
+  _lib.check(f(m._handle, d._handle, ctypes.byref(pos), ctypes.byref(vel), sh))
+  if not shapes:
+    return {"position": pos.value, "velocity": vel.value}
+  return {k: {"worlds_per_sm": n, "lpw": sh[i], "wpb": sh[i + 1], "block_bytes": sh[i + 2], "instance": TEAM_INSTANCES[sh[i + 3]]}
+          for k, n, i in (("position", pos.value, 0), ("velocity", vel.value, 4))}

@@ -453,11 +453,13 @@ int mjb_step_profile(const mjbModel* m, mjbData* d, void* stream, float* ms_out)
   for (int i = 0; i < n; i++) cudaEventDestroy(ev[i]);
   return rc;
 }
-int mjb_team_residency(const mjbModel* m, const mjbData* d, int* position_worlds, int* velocity_worlds) {
+int mjb_team_residency(const mjbModel* m, const mjbData* d, int* position_worlds, int* velocity_worlds, int* shapes) {
   if (!m || !d || !m->finalized || !d->finalized) return fail("model/data not finalized");
   if (!position_worlds || !velocity_worlds) return fail("mjb_team_residency: null output");
-  if (check(resident_worlds_position(m->dev, d->dev, position_worlds), "resident_worlds_position")) return -1;
-  if (check(resident_worlds_velocity(m->dev, d->dev, velocity_worlds, fluid(m, d)), "resident_worlds_velocity")) return -1;
+  int local[8];
+  int* sh = shapes ? shapes : local;
+  if (check(resident_worlds_position(m->dev, d->dev, position_worlds, sh), "resident_worlds_position")) return -1;
+  if (check(resident_worlds_velocity(m->dev, d->dev, velocity_worlds, sh + 4, fluid(m, d)), "resident_worlds_velocity")) return -1;
   return 0;
 }
 int mjb_set_const(const mjbModel* m, mjbData* d, int parts, int restore, void* stream) {

@@ -404,4 +404,7 @@ static TeamKernel pos_kernel(const ModelDev& m, int lpw) {
 
 size_t smem_position(const ModelDev& m, const DataDev& d) { return team_shape(m, d.wn, pos_layout(m).total, pos_kernel).block_bytes; }
 cudaError_t launch_position(const ModelDev& m, const DataDev& d, int mask, cudaStream_t s) { return team_launch(m, d, pos_layout(m).total, pos_kernel, mask, s); }
-cudaError_t resident_worlds_position(const ModelDev& m, const DataDev& d, int* worlds) { return team_resident_worlds(m, d, pos_layout(m).total, pos_kernel, worlds); }
+cudaError_t resident_worlds_position(const ModelDev& m, const DataDev& d, int* worlds, int* shape) {
+  shape[3] = 0;
+  return team_resident_worlds(m, d, pos_layout(m).total, pos_kernel, worlds, shape);
+}

@@ -123,9 +123,8 @@ static TeamKernel vel_instance(int lpw, bool bat) {
   return lpw == 8 ? k_velocity<PEXT, 8, false> : lpw == 16 ? k_velocity<PEXT, 16, false> : k_velocity<PEXT, 32, false>;
 }
 // has_gravcomp also flags free / ball joint springs (io.py put_model); tendons live in the same instantiation
-static TeamKernel vel_kernel(const ModelDev& m, int lpw) {
-  return m.has_gravcomp || m.ntendon > 0 ? vel_instance<true>(lpw, m.batched) : vel_instance<false>(lpw, m.batched);
-}
+static bool vel_pext(const ModelDev& m) { return m.has_gravcomp || m.ntendon > 0; }
+static TeamKernel vel_kernel(const ModelDev& m, int lpw) { return vel_pext(m) ? vel_instance<true>(lpw, m.batched) : vel_instance<false>(lpw, m.batched); }
 // models with fluid forces: one instance per lane count with everything the other two cover as well
 using FluidKernel = void (*)(ModelDev, DataDev, int, FluidDev);
 static FluidKernel vel_kernel_fluid(const ModelDev& m, int lpw) {
@@ -141,7 +140,8 @@ cudaError_t launch_velocity(const ModelDev& m, const DataDev& d, int mask, cudaS
   const int words = vel_layout(m).total;
   return f.has_fluid ? team_launch(m, d, words, vel_kernel_fluid, mask, s, f) : team_launch(m, d, words, vel_kernel, mask, s);
 }
-cudaError_t resident_worlds_velocity(const ModelDev& m, const DataDev& d, int* worlds, const FluidDev& f) {
+cudaError_t resident_worlds_velocity(const ModelDev& m, const DataDev& d, int* worlds, int* shape, const FluidDev& f) {
   const int words = vel_layout(m).total;
-  return f.has_fluid ? team_resident_worlds(m, d, words, vel_kernel_fluid, worlds) : team_resident_worlds(m, d, words, vel_kernel, worlds);
+  shape[3] = f.has_fluid ? 2 : vel_pext(m) ? 1 : 0;
+  return f.has_fluid ? team_resident_worlds(m, d, words, vel_kernel_fluid, worlds, shape) : team_resident_worlds(m, d, words, vel_kernel, worlds, shape);
 }

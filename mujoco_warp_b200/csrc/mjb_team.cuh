@@ -169,15 +169,17 @@ inline cudaError_t team_launch(const ModelDev& m, const DataDev& d, size_t world
   return launch(kernel_of(m, t.lpw), grid, 32 * t.wpb, t.block_bytes, team_carveout(t.block_bytes), s, m, d, mask, extra...);
 }
 
-// Worlds per SM resident at once (occupancy API) in the launch shape of d's world range.
+// Worlds per SM resident at once (occupancy API) in the launch shape of d's world range, and that shape: shape[0..2] = lanes per
+// world, warps per block, block bytes.
 template <class K>
-inline cudaError_t team_resident_worlds(const ModelDev& m, const DataDev& d, size_t world_words, TeamChooserOf<K> kernel_of, int* worlds) {
+inline cudaError_t team_resident_worlds(const ModelDev& m, const DataDev& d, size_t world_words, TeamChooserOf<K> kernel_of, int* worlds, int* shape) {
   const TeamShape t = team_shape(m, d.wn, world_words, kernel_of);
   const K kern = kernel_of(m, t.lpw);
   int blocks = 0;
   cudaError_t e = launch_configure((const void*)kern, t.block_bytes, team_carveout(t.block_bytes));
   if (e == cudaSuccess) e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&blocks, kern, 32 * t.wpb, t.block_bytes);
   *worlds = blocks * t.wpb * (32 / t.lpw);
+  shape[0] = t.lpw; shape[1] = t.wpb; shape[2] = (int)t.block_bytes;
   return e;
 }
 

@@ -246,9 +246,10 @@ size_t smem_position(const ModelDev& m, const DataDev& d);
 size_t smem_collision(const ModelDev& m, const DataDev& d);
 size_t smem_constraint(const ModelDev& m, const DataDev& d);
 size_t smem_velocity(const ModelDev& m, const DataDev& d, const FluidDev& f);
-// worlds per SM resident at once (occupancy API) in the launch shape k_position / k_velocity take for d's world range
-cudaError_t resident_worlds_position(const ModelDev& m, const DataDev& d, int* worlds);
-cudaError_t resident_worlds_velocity(const ModelDev& m, const DataDev& d, int* worlds, const FluidDev& f);
+// worlds per SM resident at once (occupancy API) in the launch shape k_position / k_velocity take for d's world range, and that
+// shape: shape[0..3] = lanes per world, warps per block, block bytes, instance (k_velocity: 0 plain, 1 PEXT, 2 fluid; k_position: 0)
+cudaError_t resident_worlds_position(const ModelDev& m, const DataDev& d, int* worlds, int* shape);
+cudaError_t resident_worlds_velocity(const ModelDev& m, const DataDev& d, int* worlds, int* shape, const FluidDev& f);
 size_t smem_solver(const ModelDev& m, const DataDev& d);
 // set_const (k_set_const.cu): body_subtreemass of worlds [0, nw); qpos swap of worlds [0, nw); set_const_0's outputs of worlds [0, nw)
 // from the position stages and factor at their qpos0; tendon_lengthspring of worlds [0, nw)
