@@ -28,6 +28,9 @@
  *   mjb_mul_m                  <- _src/support.py:153  mul_m(m, d, res, vec): res = M vec
  *   mjb_sensor_pos/vel/acc     <- _src/sensor.py:810, :1432, :2512  sensor_pos / sensor_vel / sensor_acc(m, d)
  *   mjb_energy_pos/vel         <- _src/sensor.py:2934, :3004  energy_pos / energy_vel(m, d)
+ *   mjb_read_ctrl / _sensor    <- _src/history.py:634, :718  read_ctrl / read_sensor(m, d, id, time, interp, result)
+ *   mjb_init_ctrl_history /    <- _src/history.py:796, :881  init_ctrl_history(m, d, ctrlid, times, values) /
+ *     mjb_init_sensor_history       init_sensor_history(m, d, sensorid, times, values, phase)
  *   mjb_contact_force          <- _src/support.py:445  contact_force(m, d, contact_ids, to_world_frame, force)
  *   mjb_rays                   <- _src/ray.py:1219 rays(m, d, pnt, vec, geomgroup, flg_static, bodyexclude, dist, geomid, normal) without a
  *                                 render context (every geom tested, no BVH; no height fields)
@@ -115,6 +118,20 @@ int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream);
  * both terms when ENBL_ENERGY is set; the e_potential / e_kinetic sensors are written by mjb_sensor_pos, forward, step and inverse. */
 int mjb_energy_pos(const mjbModel* m, mjbData* d, void* stream);
 int mjb_energy_vel(const mjbModel* m, mjbData* d, void* stream);
+/* history.py: actuator and sensor delays.  Data.history is bound by name ("history", (nworld, nhistory) fp32); the Model's delay fields
+ * ("actuator_history" (nu, 2) int, "actuator_historyadr", "actuator_delay", "sensor_history", "sensor_historyadr", "sensor_delay",
+ * "sensor_interval" (nsensor, 2), "sensor_history_id": the sensors with nsample > 0) and the ints "nhistory", "nactuator_history",
+ * "nsensor_history" by name as well.  forward / step read the delayed ctrl in the actuation stage, replace delayed / interval sensors after
+ * each sensor stage and insert d.ctrl once per step before time advances.
+ * read_ctrl / read_sensor: the value of actuator / sensor `id` at time[w] - delay into result (nworld) / (nworld, sensor_dim), with interp
+ * -1 (the model's), 0 zoh, 1 linear or 2 cubic; the current ctrl / sensordata for an id without a buffer.  init_*_history: the buffer of
+ * `id` (which must have nsample > 0) from times (nsample, strictly increasing; NULL: -MJ_MAXVAL stamps) and values (nworld, nsample *
+ * dim), newest last; a sensor's user slot becomes phase[w] (the last time an interval sensor was due), an actuator's is kept.  All
+ * arrays are fp32 device pointers; one kernel launch each. */
+int mjb_read_ctrl(const mjbModel* m, mjbData* d, int ctrlid, const float* time, int interp, float* result, void* stream);
+int mjb_read_sensor(const mjbModel* m, mjbData* d, int sensorid, const float* time, int interp, float* result, void* stream);
+int mjb_init_ctrl_history(const mjbModel* m, mjbData* d, int ctrlid, const float* times, const float* values, void* stream);
+int mjb_init_sensor_history(const mjbModel* m, mjbData* d, int sensorid, const float* times, const float* values, const float* phase, void* stream);
 /* support.py:445 contact_force(m, d, contact_ids, to_world_frame, force): force is (n, 6) floats, device pointers */
 int mjb_contact_force(const mjbModel* m, mjbData* d, const int* contact_ids, int n, int to_world_frame, float* force, void* stream);
 /* ray.py:1219 rays: pnt, vec (pnt_nbatch, nray, 3) fp32 device, pnt_nbatch 1 or nworld; geomgroup: 6 host ints (all -1 = no group

@@ -1,7 +1,8 @@
 """mujoco_warp_b200 -- H100-native (sm_90a) batched MuJoCo physics step behind the mujoco_warp API.
 
 Public surface mirrors /root/reference/mujoco_warp/__init__.py for the step path: put_model, put_data, make_data,
-reset_data, step, forward, the individually callable stages, potential and kinetic energy (energy_pos / energy_vel), inverse
+reset_data, step, forward, the individually callable stages, potential and kinetic energy (energy_pos / energy_vel), actuator and sensor
+delays (read_ctrl / read_sensor / init_ctrl_history / init_sensor_history), inverse
 dynamics (inverse), ray casting (ray / rays) and the per-world recomputation of derived Model constants (set_const, set_const_fixed, set_const_0, set_const_spring); `mjcf.load` stands in for mujoco's MJCF compiler.
 """
 
@@ -12,6 +13,7 @@ from ._src.forward import camlight, collision, com_pos, crb, ctrl_noise, euler, 
 from ._src.forward import fwd_position, fwd_velocity, kinematics, last_launch_count, make_constraint, solve, step, step_profile, team_residency, transmission
 from ._src.forward import energy_pos, energy_vel
 from ._src.forward import com_vel, contact_force, fwd_kinematics, get_state, implicit, mul_m, passive, rne, rungekutta4, sensor_acc, sensor_pos, sensor_vel, set_state, solve_m, step1, step2
+from ._src.history import init_ctrl_history, init_sensor_history, read_ctrl, read_sensor
 from ._src.inverse import inverse
 from ._src.ray import ray, rays
 from ._src.set_const import set_const, set_const_0, set_const_fixed, set_const_spring

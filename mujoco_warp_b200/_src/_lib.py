@@ -15,7 +15,7 @@ _PKG = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 _CSRC = os.path.join(_PKG, "csrc")
 LIB_PATH = os.environ.get("MJB_LIB", os.path.join(_PKG, "libmjb200.so"))  # MJB_LIB: A/B-test an alternative build
 HEADER_PATH = os.path.join(os.path.dirname(_PKG), "include", "mjb200.h")
-SOURCES = ["capi.cu", "k_position.cu", "k_collision.cu", "k_collision_mesh.cu", "k_constraint.cu", "k_velocity.cu", "k_solver.cu", "k_integrate.cu", "k_implicit.cu", "k_support.cu", "k_sensor.cu", "k_sensor_collision.cu", "k_ray.cu", "k_inverse.cu", "k_set_const.cu", "k_energy.cu"]
+SOURCES = ["capi.cu", "k_position.cu", "k_collision.cu", "k_collision_mesh.cu", "k_constraint.cu", "k_velocity.cu", "k_solver.cu", "k_integrate.cu", "k_implicit.cu", "k_support.cu", "k_sensor.cu", "k_sensor_collision.cu", "k_ray.cu", "k_inverse.cu", "k_set_const.cu", "k_energy.cu", "k_history.cu"]
 NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a", "--extended-lambda", "-Xcompiler", "-fPIC", "-shared"]
 
 _lib = None
@@ -114,6 +114,9 @@ def lib():
   L.mjb_rays.restype = ci
   L.mjb_set_const.argtypes = [vp, vp, ci, ci, vp]
   L.mjb_set_const.restype = ci
+  for f, args in (("mjb_read_ctrl", [vp, ci, vp]), ("mjb_read_sensor", [vp, ci, vp]), ("mjb_init_ctrl_history", [vp, vp]), ("mjb_init_sensor_history", [vp, vp, vp])):
+    getattr(L, f).argtypes = [vp, vp, ci] + args + [vp]
+    getattr(L, f).restype = ci
   L.mjb_step_profile.argtypes = [vp, vp, vp, ctypes.POINTER(ctypes.c_float)]
   L.mjb_last_launch_count.restype = ci
   _lib = L

@@ -209,9 +209,9 @@ def _state_fields(m: Model, d: Data, sig: int):
     t = {
       "TIME": lambda: d.time.reshape(nw, 1), "QPOS": lambda: d.qpos, "QVEL": lambda: d.qvel, "WARMSTART": lambda: d.qacc_warmstart,
       "CTRL": lambda: d.ctrl, "QFRC_APPLIED": lambda: d.qfrc_applied, "XFRC_APPLIED": lambda: d.xfrc_applied.reshape(nw, -1),
-      "ACT": lambda: d.act, "EQ_ACTIVE": lambda: d.eq_active.reshape(nw, -1), "MOCAP_POS": lambda: d.mocap_pos.reshape(nw, -1), "MOCAP_QUAT": lambda: d.mocap_quat.reshape(nw, -1),
+      "ACT": lambda: d.act, "HISTORY": lambda: d.history, "EQ_ACTIVE": lambda: d.eq_active.reshape(nw, -1), "MOCAP_POS": lambda: d.mocap_pos.reshape(nw, -1), "MOCAP_QUAT": lambda: d.mocap_quat.reshape(nw, -1),
     }.get(name)
-    if t is None:  # HISTORY / USERDATA: no history buffers, no user data in this build (width 0)
+    if t is None:  # USERDATA: no user data in this build (width 0)
       continue
     out.append(t())
   return out

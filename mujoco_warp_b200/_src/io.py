@@ -398,6 +398,43 @@ def _validate(mjm):
       raise NotImplementedError("site-based connect / weld equality constraints are not implemented")
   if int(np.asarray(mjm.tree_dofnum).max(initial=0)) > 64:
     raise NotImplementedError("kinematic trees with more than 64 dofs are not supported (dense per-tree Cholesky)")
+  _validate_history(mjm)
+
+
+def history_fields(mjm) -> dict:
+  """The delay / history fields of an MjModel-like object (reference types.py:1306-1329), with empty defaults for models saved
+  before they existed."""
+  nu, ns = int(mjm.nu), int(getattr(mjm, "nsensor", 0))
+  g = lambda n, shape, dt: np.asarray(getattr(mjm, n, np.zeros(shape)), dtype=dt).reshape(shape)
+  return dict(
+    actuator_history=g("actuator_history", (nu, 2), np.int32), actuator_historyadr=np.asarray(getattr(mjm, "actuator_historyadr", -np.ones(nu)), dtype=np.int32).reshape(nu),
+    actuator_delay=g("actuator_delay", (nu,), np.float64), sensor_history=g("sensor_history", (ns, 2), np.int32),
+    sensor_historyadr=np.asarray(getattr(mjm, "sensor_historyadr", -np.ones(ns)), dtype=np.int32).reshape(ns), sensor_delay=g("sensor_delay", (ns,), np.float64),
+    sensor_interval=g("sensor_interval", (ns, 2), np.float64), nhistory=int(getattr(mjm, "nhistory", 0)),
+  )
+
+
+def _validate_history(mjm):
+  """Refuses, by name, delays and intervals the history buffers would not honour: the reference silently reads the undelayed value
+  when nsample is 0 (history.py:380), and negative sizes / times have no meaning."""
+  h = history_fields(mjm)
+  names = getattr(getattr(mjm, "names", None), "__dict__", {})
+  for kind, n in (("actuator", int(mjm.nu)), ("sensor", int(getattr(mjm, "nsensor", 0)))):
+    hist, delay = h[kind + "_history"], h[kind + "_delay"]
+    period = h["sensor_interval"][:, 0] if kind == "sensor" else np.zeros(n)
+    for i in range(n):
+      what = f"{kind} {i}" + (f" ('{names[kind][i]}')" if kind in names and i < len(names[kind]) else "")
+      if hist[i, 0] < 0:
+        raise ValueError(f"{what}: nsample must be >= 0, got {hist[i, 0]}")
+      if hist[i, 1] not in (0, 1, 2):
+        raise ValueError(f"{what}: interp must be 0 (zoh), 1 (linear) or 2 (cubic), got {hist[i, 1]}")
+      if delay[i] < 0:
+        raise ValueError(f"{what}: delay must be >= 0, got {delay[i]}")
+      if period[i] < 0:
+        raise ValueError(f"{what}: interval period must be >= 0, got {period[i]}")
+      if hist[i, 0] == 0 and (delay[i] > 0 or period[i] > 0):
+        field = "delay" if delay[i] > 0 else "interval"
+        raise ValueError(f"{what}: {field} > 0 needs a history buffer (nsample > 0); with nsample = 0 it would be ignored")
 
 
 def _ptr_tensor(x: torch.Tensor) -> torch.Tensor:
@@ -416,6 +453,8 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   into `m.<field>` (in place, or by assigning a tensor with a different leading size) for domain randomisation."""
   batch_sizes = dict(batch_sizes or {})
   for name, size in batch_sizes.items():
+    if name in ("actuator_delay", "sensor_delay"):
+      raise ValueError(f"Model field {name!r} is shared by all worlds (the reference has no per-world delays); it cannot be batched.")
     if name not in _FLOAT_FIELDS and name not in _BATCHABLE_EXTRA:
       raise ValueError(f"Model field {name!r} is not a batched array field.")
     if int(size) < 1:
@@ -545,6 +584,13 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
     setattr(m, n, dev_i(x))
   m.sensor_energy_adr = dev_i(t["sensor_energy_adr"])
   m.sensor_e_potential, m.sensor_e_kinetic = t["sensor_e_potential"], t["sensor_e_kinetic"]
+  # delay / history buffers (reference types.py:1306-1329); a real MjModel's addresses are taken as given
+  hf = history_fields(mjm)
+  m.nhistory = hf.pop("nhistory")
+  for n, x in hf.items():
+    setattr(m, n, dev_i(x) if x.dtype == np.int32 else dev_f(x, batched=False))
+  m.sensor_history_id = dev_i(np.nonzero(hf["sensor_history"][:, 0] > 0)[0])  # the sensors k_history_sensor runs over
+  m._history = hf  # host copies: the public history functions check sizes against them
   m.eq_type = dev_i(mjm.eq_type if neq else np.zeros(0))
   m.eq_obj1id = dev_i(mjm.eq_obj1id if neq else np.zeros(0))
   m.eq_obj2id = dev_i(mjm.eq_obj2id if neq else np.zeros(0))
@@ -623,7 +669,8 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
     _lib.check(L.mjb_model_set_int(h, k.encode(), int(v)))
   for k, v in (("nsensorcollision", m.nsensorcollision), ("nsensorcollision_sensor", len(m.sensor_collision_id)), ("sensor_collision_epa_iterations", m.sensor_collision_epa_iterations),
                ("nsensorcollision_ccd", m.nsensorcollision_ccd), ("nsensor_energy", len(t["sensor_energy_adr"])),
-               ("sensor_e_potential", m.sensor_e_potential), ("sensor_e_kinetic", m.sensor_e_kinetic)):
+               ("sensor_e_potential", m.sensor_e_potential), ("sensor_e_kinetic", m.sensor_e_kinetic),
+               ("nhistory", m.nhistory), ("nactuator_history", int((hf["actuator_history"][:, 0] > 0).sum())), ("nsensor_history", len(m.sensor_history_id))):
     _lib.check(L.mjb_model_set_int(h, k.encode(), int(v)))
   g = np.asarray(o.gravity, dtype=np.float64)
   floats = dict(timestep=o.timestep, tolerance=tol, ls_tolerance=o.ls_tolerance, impratio_invsqrt=1.0 / np.sqrt(o.impratio),
@@ -648,7 +695,9 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
                                          "ten_J_rownnz", "ten_J_rowadr", "ten_J_colind", "tendon_adr", "tendon_num", "wrap_objid", "tendon_limited", "tendon_actfrclimited", "wrap_prm", "ten_J0",
                                          "geom_group", "geom_matid", "geom_rgba", "mat_rgba", "mesh_faceadr", "mesh_face",
                                          "geom_fluid", "body_fluid", "body_geomadr", "body_geomnum", "sensor_collision_start_adr", "sensor_collision_pair",
-                                         "sensor_collision_id", "sensor_collision_adr", "sensor_collision_flip", "actuator_acc0", "sensor_energy_adr"]
+                                         "sensor_collision_id", "sensor_collision_adr", "sensor_collision_flip", "actuator_acc0", "sensor_energy_adr",
+                                         "actuator_history", "actuator_historyadr", "actuator_delay", "sensor_history", "sensor_historyadr", "sensor_delay",
+                                         "sensor_interval", "sensor_history_id"]
                                         + [n for n, _ in _TENDON_FLOATS]):
     dev_names.setdefault(n, getattr(m, n))
   for n, x in dev_names.items():
@@ -762,7 +811,7 @@ def _data_spec(m: types.Model, nworld, naconmax, njmax, njmax_pad):
     "qfrc_fluid": (f, (nworld, nv)), "qfrc_adhesion": (f, (nworld, nv)), "qfrc_passive": (f, (nworld, nv)),
     "actuator_force": (f, (nworld, nu)), "qfrc_actuator": (f, (nworld, nv)), "qfrc_smooth": (f, (nworld, nv)), "qacc_smooth": (f, (nworld, nv)),
     "qfrc_constraint": (f, (nworld, nv)), "qfrc_inverse": (f, (nworld, nv)), "cacc": (f, (nworld, nb, 6)), "cfrc_int": (f, (nworld, nb, 6)),
-    "cfrc_ext": (f, (nworld, nb, 6)), "energy": (f, (nworld, 2)),
+    "cfrc_ext": (f, (nworld, nb, 6)), "energy": (f, (nworld, 2)), "history": (f, (nworld, m.nhistory)),
     "nacon": (i, (1,)), "ncollision": (i, (1,)), "overflow": (i, (nworld,)),
     "eq_active": (i, (nworld, getattr(m, "neq", 0))),  # the reference stores bool; int32 0/1 here (one word per flag)
     "mocap_pos": (f, (nworld, m.nmocap, 3)), "mocap_quat": (f, (nworld, m.nmocap, 4)),
@@ -799,7 +848,7 @@ _BOUND_TOP = [
   "crb", "M", "qLD", "actuator_length", "actuator_moment", "actuator_velocity", "cvel", "cdof_dot", "qfrc_bias", "qfrc_spring", "qfrc_damper",
   "qfrc_gravcomp", "qfrc_passive", "actuator_force", "qfrc_actuator", "qfrc_smooth", "qacc_smooth", "qfrc_constraint", "qfrc_inverse", "cacc", "cfrc_int",
   "ne", "nf", "nl", "nefc", "nacon", "ncollision", "solver_niter", "overflow", "moment_rownnz", "moment_rowadr", "moment_colind", "eq_active", "mocap_pos", "mocap_quat", "sensordata", "subtree_linvel", "subtree_angmom", "cfrc_ext",
-  "act", "act_dot", "ten_length", "ten_J", "ten_velocity", "qLU", "qfrc_fluid", "energy",
+  "act", "act_dot", "ten_length", "ten_J", "ten_velocity", "qLU", "qfrc_fluid", "energy", "history",
 ]
 _BOUND_EFC = ["J", "pos", "margin", "D", "vel", "aref", "frictionloss", "force", "Ma", "type", "id", "state"]
 _BOUND_CONTACT = ["dist", "pos", "frame", "includemargin", "friction", "solref", "solreffriction", "solimp", "dim", "geom", "efc_address", "worldid", "type", "geomcollisionid"]
@@ -930,7 +979,7 @@ def _bind(m: types.Model, d: types.Data, L):
 def put_data(mjm, mjd, nworld: int = 1, nconmax=None, nccdmax=None, njmax=None, njmax_nnz=None, naconmax=None, naccdmax=None, nvmax=None, m: types.Model = None) -> types.Data:
   """Moves host state (MjData-like: qpos, qvel, ctrl, qacc_warmstart, time, ...) to a device Data tiled over nworld (io.py:1890)."""
   d = make_data(mjm, nworld, nconmax, nccdmax, njmax, njmax_nnz, naconmax, naccdmax, nvmax, m=m)
-  for name in ("qpos", "qvel", "ctrl", "qacc_warmstart", "qfrc_applied", "xfrc_applied", "act"):
+  for name in ("qpos", "qvel", "ctrl", "qacc_warmstart", "qfrc_applied", "xfrc_applied", "act", "history"):
     if hasattr(mjd, name) and getattr(d, name).numel():
       src = np.asarray(getattr(mjd, name), dtype=np.float32)
       dst = getattr(d, name)
@@ -940,7 +989,8 @@ def put_data(mjm, mjd, nworld: int = 1, nconmax=None, nccdmax=None, njmax=None, 
 
 
 def reset_data(m: types.Model, d: types.Data):
-  """Resets every world to qpos0 with zero velocity/ctrl/time (reference io.py:2435, all worlds)."""
+  """Resets every world to qpos0 with zero velocity/ctrl/time (reference io.py:2435, all worlds).  d.history (the actuator and sensor
+  delay buffers) is left untouched, as the reference leaves it; refill it with init_ctrl_history / init_sensor_history."""
   mjm = m._mjm
   d.qpos.copy_(torch.from_numpy(np.tile(np.asarray(mjm.qpos0, dtype=np.float32), (d.nworld, 1))))
   for n in ("qvel", "ctrl", "qacc_warmstart", "qacc", "qfrc_applied", "xfrc_applied", "time", "act", "act_dot"):
@@ -1012,6 +1062,8 @@ def get_data_into(result, mjm, d: types.Data, world_id: int = 0):
   nefc = min(int(d.nefc[w].cpu()), d.njmax)
   for name in _GET_FIELDS:
     setattr(result, name, getattr(d, name)[w].cpu().numpy().astype(np.float64))
+  if d.history.shape[1] > 0:  # reference io.py:2322
+    result.history = d.history[w].cpu().numpy().astype(np.float64)
   result.qM = d.M[w].cpu().numpy().astype(np.float64)
   result.M = result.qM
   result.time = float(d.time[w].cpu())

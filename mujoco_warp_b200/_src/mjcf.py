@@ -288,6 +288,40 @@ def _geom_aabb(gtype, size):
 # ----------------------------------------------------------------------------------------------
 
 _ACT_TAGS = ("general", "motor", "position", "velocity", "intvelocity", "damper", "cylinder", "muscle", "adhesion")
+# delay / history attributes of actuators and sensors; interp keywords as in the reference's history.py:88 (0 zoh, 1 linear, 2 cubic)
+_HISTORY_KEYS = ("nsample", "interp", "delay", "interval")
+_INTERP = {"zoh": 0, "linear": 1, "cubic": 2}
+
+
+def _history_attrs(a, what, interval):
+  """((nsample, interp), delay, (period, phase)) of an actuator or sensor element.  Range checks (negative values, a delay or interval
+  without samples) are io._validate's, so that they also hold for models that do not come from this compiler."""
+  interp = a.get("interp", "zoh")
+  if interp not in _INTERP:
+    raise ValueError(f"{what}: interp must be one of {sorted(_INTERP)}, got '{interp}'")
+  iv = np.zeros(2)
+  if interval and "interval" in a:
+    v = _vec(a["interval"])
+    if v.size not in (1, 2):
+      raise ValueError(f"{what}: interval takes 'period [phase]', got '{a['interval']}'")
+    iv[: v.size] = v
+  return (int(a.get("nsample", 0)), _INTERP[interp]), float(a.get("delay", 0.0)), iv
+
+
+def set_history_layout(m):
+  """actuator_historyadr / sensor_historyadr / nhistory of the delay buffers (reference history.py): one buffer per actuator or sensor
+  with nsample > 0, [user, cursor, times[n], values[n * dim]] (dim 1 for actuators), actuators in index order, then sensors; -1 for
+  the others."""
+  adr = 0
+  out = {}
+  for kind, hist, dims in (("actuator", m.actuator_history, np.ones(len(m.actuator_history), dtype=int)), ("sensor", m.sensor_history, m.sensor_dim)):
+    a = -np.ones(len(hist), dtype=np.int32)
+    for i, (n, dim) in enumerate(zip(np.asarray(hist).reshape(-1, 2)[:, 0], np.asarray(dims).reshape(-1))):
+      if n > 0:
+        a[i] = adr
+        adr += 2 + int(n) * (1 + int(dim))
+    out[kind] = a
+  m.actuator_historyadr, m.sensor_historyadr, m.nhistory = out["actuator"], out["sensor"], adr
 
 
 class _Defaults:
@@ -1238,9 +1272,12 @@ def compile_xml(root):
   m.actuator_actnum = np.zeros(nu, dtype=np.int32)
   m.actuator_actearly = np.zeros(nu, dtype=bool)
   m.names.actuator = []
+  m.actuator_history = np.zeros((nu, 2), dtype=np.int32)
+  m.actuator_delay = np.zeros(nu)
   dyn_names = {"none": C.DYN_NONE, "integrator": C.DYN_INTEGRATOR, "filter": C.DYN_FILTER, "filterexact": C.DYN_FILTEREXACT}
   for i, (tag, a) in enumerate(acts):
     m.names.actuator.append(a.get("name", f"actuator{i}"))
+    m.actuator_history[i], m.actuator_delay[i], _ = _history_attrs(a, f"actuator '{m.names.actuator[-1]}'", interval=False)
     if "tendon" in a:
       m.actuator_trntype[i] = C.TRN_TENDON
       m.actuator_trnid[i, 0] = m.names.tendon.index(a["tendon"])
@@ -1492,8 +1529,12 @@ def compile_xml(root):
     else:
       otype, lst = objkind[kind]
       oid = getattr(m.names, lst).index(e.get(kind))
-    sens.append(dict(name=e.get("name", f"sensor{len(sens)}"), type=stype, objtype=otype, objid=oid, reftype=rtype, refid=rid, dim=dim, datatype=datatype, needstage=stage,
-                     cutoff=float(e.get("cutoff", 0.0)), noise=float(e.get("noise", 0.0))))
+    sname = e.get("name", f"sensor{len(sens)}")
+    ha = {k: v for k, v in dflt.resolve("sensor", e.get("class", "main")).items() if k in _HISTORY_KEYS}
+    ha.update(e.attrib)
+    hist, delay, interval = _history_attrs(ha, f"sensor '{sname}'", interval=True)
+    sens.append(dict(name=sname, type=stype, objtype=otype, objid=oid, reftype=rtype, refid=rid, dim=dim, datatype=datatype, needstage=stage,
+                     cutoff=float(e.get("cutoff", 0.0)), noise=float(e.get("noise", 0.0)), history=hist, delay=delay, interval=interval))
   m.nsensor = len(sens)
   m.sensor_unsupported = unsupported  # put_model refuses these (they would silently read zero otherwise)
   m.names.sensor = [x["name"] for x in sens]
@@ -1503,6 +1544,10 @@ def compile_xml(root):
   m.sensor_noise = np.array([x["noise"] for x in sens], dtype=np.float64).reshape(m.nsensor)
   m.sensor_adr = (np.concatenate(([0], np.cumsum(m.sensor_dim)[:-1])) if m.nsensor else np.zeros(0)).astype(np.int32)
   m.nsensordata = int(m.sensor_dim.sum()) if m.nsensor else 0
+  m.sensor_history = np.array([x["history"] for x in sens], dtype=np.int32).reshape(m.nsensor, 2)
+  m.sensor_delay = np.array([x["delay"] for x in sens], dtype=np.float64).reshape(m.nsensor)
+  m.sensor_interval = np.array([x["interval"] for x in sens], dtype=np.float64).reshape(m.nsensor, 2)
+  set_history_layout(m)
 
   # ---- keyframes
   keys = []

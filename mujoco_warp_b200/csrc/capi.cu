@@ -16,6 +16,7 @@ struct mjbModel {
   SensorCollisionDev sc;
   SetConstDev setc;  // actuator_acc0 and the meaninertia output, bound by name; qpos_save stays null here (the Data's)
   EnergyDev en;      // the energy sensors; energy stays null here (the Data's: energy() below)
+  HistoryDev hist;   // the delay fields; history and ctrl_delayed stay null here (the Data's: history() below)
   bool finalized;
 };
 struct mjbData {
@@ -33,6 +34,8 @@ struct mjbData {
   float* qfrc_fluid;    // Data.qfrc_fluid, (nworld, nv), bound by name; passed to the fluid kernels in FluidDev
   float* qpos_save;     // (nworld, nq) d.qpos while mjb_set_const runs the position stages at qpos0 / qpos_spring
   float* energy;        // Data.energy, (nworld, 2), bound by name; passed to k_energy in EnergyDev
+  float* history;       // Data.history, (nworld, nhistory), bound by name; passed to k_history in HistoryDev
+  float* ctrl_delayed;  // (nworld, nu) the delayed ctrl the actuation stage reads; allocated for models with actuator delays only
 };
 
 namespace {
@@ -49,6 +52,8 @@ constexpr size_t kMaxSmem = 227 * 1024;
 static FluidDev fluid(const mjbModel* m, const mjbData* d) { FluidDev f = m->fluid; f.qfrc_fluid = d->qfrc_fluid; return f; }
 // The energy sensors of a model bound to a Data's energy
 static EnergyDev energy(const mjbModel* m, const mjbData* d) { EnergyDev e = m->en; e.energy = d->energy; return e; }
+// The delay fields of a model bound to a Data's history buffers
+static HistoryDev history(const mjbModel* m, const mjbData* d) { HistoryDev h = m->hist; h.history = d->history; h.ctrl_delayed = d->ctrl_delayed; return h; }
 
 extern "C" {
 
@@ -63,6 +68,7 @@ mjbModel* mjb_model_create(void) {
   memset(&m->sc, 0, sizeof(SensorCollisionDev));
   memset(&m->setc, 0, sizeof(SetConstDev));
   memset(&m->en, 0, sizeof(EnergyDev));
+  memset(&m->hist, 0, sizeof(HistoryDev));
   m->finalized = false;
   return m;
 }
@@ -80,6 +86,9 @@ int mjb_model_set_int(mjbModel* m, const char* name, int v) {
 #undef X
 #define X(n) if (!strcmp(name, #n)) { m->en.n = v; return 0; }
   MJB_ENERGY_INTS(X)
+#undef X
+#define X(n) if (!strcmp(name, #n)) { m->hist.n = v; return 0; }
+  MJB_HISTORY_INTS(X)
 #undef X
   return fail(std::string("unknown model int field: ") + name);
 }
@@ -106,6 +115,10 @@ int mjb_model_set_array_batched(mjbModel* m, const char* name, const void* p, in
 #undef X
 #define X(n) if (!strcmp(name, #n)) { if (nbatch != 1) return fail(std::string("shared by all worlds (not batched): ") + name); m->en.n = (const int*)p; return 0; }
   MJB_ENERGY_IARRS(X)
+#undef X
+#define X(n) if (!strcmp(name, #n)) { if (nbatch != 1) return fail(std::string("shared by all worlds (not batched): ") + name); m->hist.n = (decltype(m->hist.n))p; return 0; }
+  MJB_HISTORY_IARRS(X)
+  MJB_HISTORY_FARRS(X)
 #undef X
   if (!strcmp(name, "actuator_acc0")) { m->setc.actuator_acc0 = (float*)p; m->setc.nb_actuator_acc0 = nbatch; return 0; }
   if (!strcmp(name, "meaninertia")) {
@@ -143,6 +156,10 @@ int mjb_model_finalize(mjbModel* m) {
 #define X(n) if (!m->en.n) return fail(std::string("model array not set: ") + #n);
   MJB_ENERGY_IARRS(X)
 #undef X
+#define X(n) if (!m->hist.n) return fail(std::string("model array not set: ") + #n);
+  MJB_HISTORY_IARRS(X)
+  MJB_HISTORY_FARRS(X)
+#undef X
   if (m->dev.nv <= 0 || m->dev.nbody <= 0) return fail("model has no dofs/bodies");
   if (m->dev.solver != SOL_NEWTON && m->dev.solver != SOL_CG) return fail("only the Newton and CG solvers are implemented");
   if (m->dev.cone != CONE_PYRAMIDAL && m->dev.cone != CONE_ELLIPTIC) return fail("unknown friction cone type");
@@ -165,6 +182,8 @@ mjbData* mjb_data_create(int nworld, int nconmax, int naconmax, int njmax, int n
   d->qfrc_fluid = nullptr;
   d->qpos_save = nullptr;
   d->energy = nullptr;
+  d->history = nullptr;
+  d->ctrl_delayed = nullptr;
   return d;
 }
 void mjb_data_destroy(mjbData* d) {
@@ -175,6 +194,7 @@ void mjb_data_destroy(mjbData* d) {
   if (d->inv_qacc) cudaFree(d->inv_qacc);
   if (d->rk) cudaFree(d->rk);
   if (d->qpos_save) cudaFree(d->qpos_save);
+  if (d->ctrl_delayed) cudaFree(d->ctrl_delayed);
   if (d->nsplit > 1) {
     for (int i = 0; i < d->nsplit; i++) { cudaStreamDestroy(d->aux[i]); cudaEventDestroy(d->ev_join[i]); }
     cudaEventDestroy(d->ev_fork);
@@ -189,6 +209,7 @@ int mjb_data_set_array(mjbData* d, const char* name, void* p) {
   if (!strcmp(name, "qfrc_inverse")) { d->qfrc_inverse = (float*)p; return 0; }
   if (!strcmp(name, "qfrc_fluid")) { d->qfrc_fluid = (float*)p; return 0; }
   if (!strcmp(name, "energy")) { d->energy = (float*)p; return 0; }
+  if (!strcmp(name, "history")) { d->history = (float*)p; return 0; }
 #define X(n) if (!strcmp(name, #n)) { d->dev.n = (float*)p; return 0; }
   MJB_DATA_FARRS(X)
 #undef X
@@ -206,6 +227,7 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
   if (!d->qfrc_inverse) return fail("data array not set: qfrc_inverse");
   if (!d->qfrc_fluid) return fail("data array not set: qfrc_fluid");
   if (!d->energy) return fail("data array not set: energy");
+  if (!d->history) return fail("data array not set: history");
   if (d->dev.nv_pad < m->dev.nv) return fail("nv_pad < nv");
   if (check(cudaMalloc(&d->dev.world_conadr, sizeof(int) * (size_t)d->dev.nworld), "cudaMalloc(world_conadr)")) return -1;
   if (check(cudaMalloc(&d->dev.world_ncon, sizeof(int) * (size_t)d->dev.nworld), "cudaMalloc(world_ncon)")) return -1;
@@ -217,6 +239,8 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
   if (!d->inv_qacc && check(cudaMalloc(&d->inv_qacc, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nv > 0 ? m->dev.nv : 1)), "cudaMalloc(inv_qacc)")) return -1;
   // set_const's save buffer, so that mjb_set_const allocates nothing (and can be captured in a graph)
   if (!d->qpos_save && check(cudaMalloc(&d->qpos_save, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nq > 0 ? m->dev.nq : 1)), "cudaMalloc(qpos_save)")) return -1;
+  if (m->hist.nactuator_history > 0 && !d->ctrl_delayed &&
+      check(cudaMalloc(&d->ctrl_delayed, sizeof(float) * (size_t)d->dev.nworld * (size_t)m->dev.nu), "cudaMalloc(ctrl_delayed)")) return -1;
   if (m->dev.integrator == INT_RK4 && !d->rk &&
       check(cudaMalloc(&d->rk, sizeof(float) * (size_t)d->dev.nworld * (size_t)(m->dev.nq + 3 * m->dev.nv + 2 * m->dev.na + 1)), "cudaMalloc(rk)")) return -1;
   const size_t smem[6] = {smem_position(m->dev, d->dev), smem_collision(m->dev, d->dev), smem_constraint(m->dev, d->dev),
@@ -257,6 +281,24 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
   g_launches = 0;
 #define MJB_LAUNCH(call) do { if (check((call), #call)) return -1; } while (0)
 
+// The Data the actuation stage reads for dd's world range (forward.py:1161-1165): with actuator delays its ctrl is the delayed one,
+// which k_history_ctrl_read writes first.  Every other kernel keeps reading d.ctrl.
+static int actuation_data(const mjbModel* m, const mjbData* d, const DataDev& dd, cudaStream_t s, DataDev* out) {
+  *out = dd;
+  if (m->hist.nactuator_history == 0) return 0;
+  out->ctrl = d->ctrl_delayed;
+  return check(launch_history_ctrl_read(m->dev, dd, history(m, d), s), "launch_history_ctrl_read");
+}
+// The actuator buffers take d.ctrl at d.time before the integrator advances it (forward.py:320, _advance)
+static cudaError_t history_ctrl_insert(const mjbModel* m, const mjbData* d, const DataDev& dd, cudaStream_t s) {
+  return m->hist.nactuator_history > 0 ? launch_history_ctrl_insert(m->dev, dd, history(m, d), s) : cudaSuccess;
+}
+// The sensors of `stages` with a buffer report their delayed / held value and record the fresh one (sensor.py:956, :1502, :2765)
+static cudaError_t history_sensor(const mjbModel* m, const mjbData* d, const DataDev& dd, int stages, cudaStream_t s) {
+  if (m->hist.nsensor_history == 0 || (m->dev.disableflags & DSBL_SENSOR)) return cudaSuccess;
+  return launch_history_sensor(m->dev, dd, history(m, d), stages, s);
+}
+
 int mjb_kinematics(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_KINEMATICS, s)); return 0; }
 int mjb_com_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_COM_POS, s)); return 0; }
 int mjb_camlight(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_CAMLIGHT, s)); return 0; }
@@ -270,7 +312,13 @@ int mjb_make_constraint(const mjbModel* m, mjbData* d, void* stream) {
   return 0;
 }
 int mjb_fwd_velocity(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_VELOCITY, s, fluid(m, d))); return 0; }
-int mjb_fwd_actuation(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_ACTUATION, s, fluid(m, d))); return 0; }
+int mjb_fwd_actuation(const mjbModel* m, mjbData* d, void* stream) {
+  MJB_ENTER();
+  DataDev da;
+  if (actuation_data(m, d, d->dev, s, &da)) return -1;
+  MJB_LAUNCH(launch_velocity(m->dev, da, STG_ACTUATION, s, fluid(m, d)));
+  return 0;
+}
 int mjb_fwd_acceleration(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_ACCELERATION, s, fluid(m, d))); return 0; }
 int mjb_factor_m(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_FACTOR_ONLY, s, fluid(m, d))); return 0; }
 int mjb_com_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_velocity(m->dev, d->dev, STG_COMVEL, s, fluid(m, d))); return 0; }
@@ -323,14 +371,30 @@ int mjb_sensor_pos(const mjbModel* m, mjbData* d, void* stream) {
   MJB_ENTER();
   MJB_LAUNCH(launch_sensor(m->dev, d->dev, 1, s, m->sc));
   MJB_LAUNCH(launch_energy(m->dev, d->dev, energy(m, d), energy_sensor_parts(m), s));
+  MJB_LAUNCH(history_sensor(m, d, d->dev, 1, s));
   return 0;
 }
 int mjb_energy_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_energy(m->dev, d->dev, energy(m, d), ENERGY_POT, s)); return 0; }
 int mjb_energy_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_energy(m->dev, d->dev, energy(m, d), ENERGY_KIN, s)); return 0; }
-int mjb_sensor_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 2, s, m->sc)); return 0; }
-int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_sensor(m->dev, d->dev, 4, s, m->sc)); return 0; }
+int mjb_sensor_vel(const mjbModel* m, mjbData* d, void* stream) {
+  MJB_ENTER();
+  MJB_LAUNCH(launch_sensor(m->dev, d->dev, 2, s, m->sc));
+  MJB_LAUNCH(history_sensor(m, d, d->dev, 2, s));
+  return 0;
+}
+int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream) {
+  MJB_ENTER();
+  MJB_LAUNCH(launch_sensor(m->dev, d->dev, 4, s, m->sc));
+  MJB_LAUNCH(history_sensor(m, d, d->dev, 4, s));
+  return 0;
+}
 int mjb_solve(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_solver(m->dev, d->dev, s)); return 0; }
-int mjb_euler(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_integrate(m->dev, d->dev, INT_EULER, s, fluid(m, d))); return 0; }
+int mjb_euler(const mjbModel* m, mjbData* d, void* stream) {
+  MJB_ENTER();
+  MJB_LAUNCH(history_ctrl_insert(m, d, d->dev, s));
+  MJB_LAUNCH(launch_integrate(m->dev, d->dev, INT_EULER, s, fluid(m, d)));
+  return 0;
+}
 
 // which stages a pipeline call runs
 enum { RUN_POSITION = 1, RUN_VELOCITY = 2, RUN_SOLVER = 4, RUN_EULER = 8, RUN_INVERSE = 16 };
@@ -357,7 +421,9 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
     MJB_MARK(2);
   }
   if (what & RUN_VELOCITY) {
-    MJB_LAUNCH(launch_velocity(m->dev, dd, STG_VELOCITY | STG_ACTUATION | STG_ACCELERATION, s, fluid(m, d)));
+    DataDev da;
+    if (actuation_data(m, d, dd, s, &da)) return -1;
+    MJB_LAUNCH(launch_velocity(m->dev, da, STG_VELOCITY | STG_ACTUATION | STG_ACCELERATION, s, fluid(m, d)));
     MJB_MARK(3);
   }
   if (what & RUN_SOLVER) {
@@ -366,6 +432,7 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
     if (m->dev.nsensor > 0) MJB_LAUNCH(launch_sensor(m->dev, dd, 7, s, m->sc));
     // energy after the sensors (the reference's energy_pos / energy_vel, forward.py:1327-1356): its inputs are final since fwd_velocity
     MJB_LAUNCH(launch_energy(m->dev, dd, energy(m, d), energy_forward_parts(m), s));
+    MJB_LAUNCH(history_sensor(m, d, dd, 7, s));  // after every kernel that writes sensordata
     MJB_MARK(4);
   }
   if (what & RUN_INVERSE) {
@@ -379,9 +446,11 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
       MJB_LAUNCH(launch_sensor(m->dev, ds, 7, s, m->sc));
     }
     MJB_LAUNCH(launch_energy(m->dev, dd, energy(m, d), energy_sensor_parts(m), s));  // inverse computes energy only for its sensors
+    MJB_LAUNCH(history_sensor(m, d, dd, 7, s));
   }
   if (what & RUN_EULER) {
     if (m->dev.integrator == INT_IMPLICIT && smem_implicit(m->dev) > kMaxSmem) return fail("implicit integrator: the velocity-derivative scratch (18 x nbody x 32 floats) exceeds one block's shared memory");
+    MJB_LAUNCH(history_ctrl_insert(m, d, dd, s));
     MJB_LAUNCH(launch_integrate(m->dev, dd, -1, s, fluid(m, d)));
     MJB_MARK(5);
   }
@@ -426,6 +495,7 @@ static int rk4_after_forward(const mjbModel* m, mjbData* d, cudaStream_t s) {
   if (!d->rk) return fail("Runge-Kutta scratch missing: data was finalized against a model whose integrator is not RK4");
   for (int stage = 0; stage < 4; stage++) {
     if (stage > 0 && pipeline(m, d, RUN_POSITION | RUN_VELOCITY | RUN_SOLVER, s)) return -1;
+    if (stage == 3) MJB_LAUNCH(history_ctrl_insert(m, d, d->dev, s));  // once, before the last stage advances d.time
     MJB_LAUNCH(launch_rk_stage(m->dev, d->dev, d->rk, stage, s));
   }
   return 0;
@@ -516,6 +586,42 @@ int mjb_set_const(const mjbModel* m, mjbData* d, int parts, int restore, void* s
     MJB_LAUNCH(launch_velocity(md, d->dev, STG_FACTOR_ONLY, s, fluid(m, d)));
   }
   return 0;
+}
+
+// history.py:634-925 read_ctrl / read_sensor / init_ctrl_history / init_sensor_history, every world
+static int history_check(const mjbModel* m, int sensor, int id, bool need_buffer) {
+  const int count = sensor ? m->dev.nsensor : m->dev.nu;
+  const char* what = sensor ? "sensor" : "actuator";
+  if (id < 0 || id >= count) return fail(std::string(what) + " id " + std::to_string(id) + " out of range [0, " + std::to_string(count) + ")");
+  if (need_buffer) {
+    int n = 0;
+    if (check(cudaMemcpy(&n, (sensor ? m->hist.sensor_history : m->hist.actuator_history) + 2 * id, sizeof(int), cudaMemcpyDeviceToHost), "cudaMemcpy(history)")) return -1;
+    if (n <= 0) return fail(std::string(what) + " " + std::to_string(id) + " has no history buffer (nsample = 0)");
+  }
+  return 0;
+}
+static int history_read(const mjbModel* m, mjbData* d, int sensor, int id, const float* time, int interp, float* result, void* stream) {
+  MJB_ENTER();
+  if (!time || !result) return fail("null array");
+  if (interp < -1 || interp > 2) return fail("interp must be -1 (the model's), 0 (zoh), 1 (linear) or 2 (cubic), got " + std::to_string(interp));
+  if (history_check(m, sensor, id, false)) return -1;
+  MJB_LAUNCH(launch_history_read(m->dev, d->dev, history(m, d), sensor, id, time, interp, result, s));
+  return 0;
+}
+static int history_init(const mjbModel* m, mjbData* d, int sensor, int id, const float* times, const float* values, const float* phase, void* stream) {
+  MJB_ENTER();
+  if (!values || (sensor && !phase)) return fail("null array");
+  if (history_check(m, sensor, id, true)) return -1;
+  MJB_LAUNCH(launch_history_init(m->dev, d->dev, history(m, d), sensor, id, times, values, phase, s));
+  return 0;
+}
+int mjb_read_ctrl(const mjbModel* m, mjbData* d, int ctrlid, const float* time, int interp, float* result, void* stream) { return history_read(m, d, 0, ctrlid, time, interp, result, stream); }
+int mjb_read_sensor(const mjbModel* m, mjbData* d, int sensorid, const float* time, int interp, float* result, void* stream) { return history_read(m, d, 1, sensorid, time, interp, result, stream); }
+int mjb_init_ctrl_history(const mjbModel* m, mjbData* d, int ctrlid, const float* times, const float* values, void* stream) {
+  return history_init(m, d, 0, ctrlid, times, values, nullptr, stream);
+}
+int mjb_init_sensor_history(const mjbModel* m, mjbData* d, int sensorid, const float* times, const float* values, const float* phase, void* stream) {
+  return history_init(m, d, 1, sensorid, times, values, phase, stream);
 }
 
 int mjb_ctrl_noise(const mjbModel* m, mjbData* d, const float* ctrl_center, int step, float noise_std, float noise_rate, void* stream) {

@@ -172,6 +172,28 @@ struct EnergyDev {
 // (forward with ENBL_ENERGY off: the sensors report, Data.energy ends at zero)
 enum { ENERGY_POT = 1, ENERGY_KIN = 2, ENERGY_SENSOR = 4, ENERGY_ZERO = 8 };
 
+// ---------------------------------------------------------------- actuator and sensor delays (k_history.cu, mjb_history.cuh)
+// The delay / history fields of the Model and Data.history, passed as one extra argument to the k_history kernels only, for the same
+// reason as FluidDev.  Buffers are laid out as [user, cursor, times[n], values[n * dim]] at *_historyadr of each world's row.
+#define MJB_HISTORY_INTS(X) X(nhistory) X(nactuator_history) X(nsensor_history)
+#define MJB_HISTORY_IARRS(X) X(actuator_history) X(actuator_historyadr) X(sensor_history) X(sensor_historyadr) X(sensor_history_id)
+#define MJB_HISTORY_FARRS(X) X(actuator_delay) X(sensor_delay) X(sensor_interval)
+struct HistoryDev {
+  int nhistory;                                 // floats of history per world
+  int nactuator_history;                        // actuators with nsample > 0
+  int nsensor_history;                         // sensors with nsample > 0
+  const int* __restrict__ actuator_history;     // (nu, 2) nsample, interp
+  const int* __restrict__ actuator_historyadr;  // (nu) buffer address or -1
+  const int* __restrict__ sensor_history;       // (nsensor, 2)
+  const int* __restrict__ sensor_historyadr;    // (nsensor)
+  const int* __restrict__ sensor_history_id;    // (nsensor_history) the sensors with nsample > 0
+  const float* __restrict__ actuator_delay;     // (nu)
+  const float* __restrict__ sensor_delay;       // (nsensor)
+  const float* __restrict__ sensor_interval;    // (nsensor, 2) period, phase
+  float* __restrict__ history;                  // Data.history (nworld, nhistory)
+  float* __restrict__ ctrl_delayed;             // (nworld, nu) the ctrl k_velocity's actuation reads (mjb_data_finalize allocates it)
+};
+
 // ---------------------------------------------------------------- enums (MuJoCo values; see constants.py)
 enum { JNT_FREE = 0, JNT_BALL = 1, JNT_SLIDE = 2, JNT_HINGE = 3 };
 enum { GEOM_PLANE = 0, GEOM_HFIELD, GEOM_SPHERE, GEOM_CAPSULE, GEOM_ELLIPSOID, GEOM_CYLINDER, GEOM_BOX, GEOM_MESH };
@@ -261,3 +283,13 @@ size_t smem_set_const(const ModelDev& m);
 // energy (k_energy.cu): the ENERGY_* parts of d's world range
 cudaError_t launch_energy(const ModelDev& m, const DataDev& d, const EnergyDev& e, int parts, cudaStream_t s);
 size_t smem_integrate(const ModelDev& m);
+// actuator and sensor delays (k_history.cu), each over d's world range: the delayed ctrl into h.ctrl_delayed; d.ctrl inserted at
+// d.time; the sensors of `stages` (1 pos, 2 vel, 4 acc) replaced by their delayed / held values, the fresh ones inserted
+cudaError_t launch_history_ctrl_read(const ModelDev& m, const DataDev& d, const HistoryDev& h, cudaStream_t s);
+cudaError_t launch_history_ctrl_insert(const ModelDev& m, const DataDev& d, const HistoryDev& h, cudaStream_t s);
+cudaError_t launch_history_sensor(const ModelDev& m, const DataDev& d, const HistoryDev& h, int stages, cudaStream_t s);
+// the public history functions, every world: one actuator's or sensor's value at time[w] - delay into result (nworld, dim); one
+// buffer filled from times (n, or null: -MJ_MAXVAL stamps) and values (nworld, n * dim), its user slot set to phase[w] (sensors) or kept
+cudaError_t launch_history_read(const ModelDev& m, const DataDev& d, const HistoryDev& h, int sensor, int id, const float* time, int interp, float* result, cudaStream_t s);
+cudaError_t launch_history_init(const ModelDev& m, const DataDev& d, const HistoryDev& h, int sensor, int id, const float* times, const float* values, const float* phase,
+                                cudaStream_t s);
