@@ -42,6 +42,7 @@
  *                                                      then advance.  Error for Euler / RK4 models: the scratch is sized per integrator)
  *   mjb_ctrl_noise             <- _src/cli.py:103      _ctrl_noise (harness kernel, untimed in testspeed)
  *   mjb_set_const              <- _src/set_const.py:613-950 set_const_fixed / set_const_0 / set_const_spring / set_const(m, d, restore)
+ *   mjb_set_length_range       <- _src/set_const.py:952 set_length_range(m, d, index)
  *
  * Conventions: plain pointers and sizes only (no torch / warp types).  All array pointers are DEVICE
  * pointers owned by the caller for the lifetime of the handle (borrowed, never freed here).  Layout is
@@ -161,6 +162,11 @@ int mjb_implicit(const mjbModel* m, mjbData* d, void* stream);
 #define MJB_SET_CONST_0 2
 #define MJB_SET_CONST_SPRING 4
 int mjb_set_const(const mjbModel* m, mjbData* d, int parts, int restore, void* stream);
+/* set_const.py:573-607, 952-985: actuator_lengthrange from the joint and tendon limits.  An actuator on a limited joint or limited fixed
+ * tendon gets the limit range times gear[0] (ends swapped for a negative gear); every other actuator gets (0, 0).  Every actuator is
+ * written whatever index is, as the reference does; index must be -1 or an actuator id.  Entry i of a batched actuator_lengthrange is
+ * computed from world i (jnt_range / tendon_range / gear read as world i sees them); nb > nworld is an error.  One kernel, stream-ordered. */
+int mjb_set_length_range(const mjbModel* m, mjbData* d, int index, void* stream);
 /* ctrl <- OU noise around ctrl_center (device array of nu floats, or NULL), reference cli.py:103-145 */
 int mjb_ctrl_noise(const mjbModel* m, mjbData* d, const float* ctrl_center, int step, float noise_std, float noise_rate, void* stream);
 

@@ -114,6 +114,8 @@ def lib():
   L.mjb_rays.restype = ci
   L.mjb_set_const.argtypes = [vp, vp, ci, ci, vp]
   L.mjb_set_const.restype = ci
+  L.mjb_set_length_range.argtypes = [vp, vp, ci, vp]
+  L.mjb_set_length_range.restype = ci
   for f, args in (("mjb_read_ctrl", [vp, ci, vp]), ("mjb_read_sensor", [vp, ci, vp]), ("mjb_init_ctrl_history", [vp, vp]), ("mjb_init_sensor_history", [vp, vp, vp])):
     getattr(L, f).argtypes = [vp, vp, ci] + args + [vp]
     getattr(L, f).restype = ci

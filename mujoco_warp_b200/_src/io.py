@@ -42,7 +42,7 @@ _TENDON_FLOATS = (("tendon_range", 2), ("tendon_margin", 1), ("tendon_stiffness"
                   ("tendon_length0", 1), ("tendon_invweight0", 1), ("tendon_solref_lim", 2), ("tendon_solimp_lim", 5), ("tendon_solref_fri", 2), ("tendon_solimp_fri", 5), ("tendon_actfrcrange", 2))
 # float fields outside _FLOAT_FIELDS that carry the reference's `*` leading dimension as well
 _BATCHABLE_EXTRA = ("eq_solref", "eq_solimp", "eq_data", "pair_friction", "pair_solref", "pair_solreffriction", "pair_solimp", "pair_margin", "pair_gap",
-                    "actuator_dynprm", "actuator_actrange", "geom_rgba", "mat_rgba", "actuator_acc0") + tuple(n for n, _ in _TENDON_FLOATS)
+                    "actuator_dynprm", "actuator_actrange", "geom_rgba", "mat_rgba", "actuator_acc0", "actuator_lengthrange") + tuple(n for n, _ in _TENDON_FLOATS)
 _SIZES = ["nq", "nv", "nu", "na", "nbody", "njnt", "ngeom", "nsite", "ncam", "nlight", "ntree", "nkey", "nmocap", "neq", "ntendon", "nflex"]
 
 _SUPPORTED_PAIRS = {
@@ -365,13 +365,20 @@ def _validate(mjm):
     raise NotImplementedError(f"enable flag(s) {names} are not implemented (contact override, fwdinv, sleeping)")
   if getattr(mjm, "nu", 0):
     gt, bt = np.asarray(mjm.actuator_gaintype), np.asarray(mjm.actuator_biastype)
-    if not np.isin(gt, (C.GAIN_FIXED, C.GAIN_AFFINE)).all():
-      raise NotImplementedError(f"actuator gain type(s) {sorted(set(gt[~np.isin(gt, (C.GAIN_FIXED, C.GAIN_AFFINE))].tolist()))} are not implemented (fixed and affine are)")
-    if not np.isin(bt, (C.BIAS_NONE, C.BIAS_AFFINE)).all():
-      raise NotImplementedError(f"actuator bias type(s) {sorted(set(bt[~np.isin(bt, (C.BIAS_NONE, C.BIAS_AFFINE))].tolist()))} are not implemented (none and affine are)")
+    if not np.isin(gt, (C.GAIN_FIXED, C.GAIN_AFFINE, C.GAIN_MUSCLE)).all():
+      raise NotImplementedError(f"actuator gain type(s) {sorted(set(gt[~np.isin(gt, (C.GAIN_FIXED, C.GAIN_AFFINE, C.GAIN_MUSCLE))].tolist()))} are not implemented (fixed, affine and muscle are)")
+    if not np.isin(bt, (C.BIAS_NONE, C.BIAS_AFFINE, C.BIAS_MUSCLE)).all():
+      raise NotImplementedError(f"actuator bias type(s) {sorted(set(bt[~np.isin(bt, (C.BIAS_NONE, C.BIAS_AFFINE, C.BIAS_MUSCLE))].tolist()))} are not implemented (none, affine and muscle are)")
     dyn = np.asarray(getattr(mjm, "actuator_dyntype", np.zeros(mjm.nu)))
-    if not np.isin(dyn, (C.DYN_NONE, C.DYN_INTEGRATOR, C.DYN_FILTER, C.DYN_FILTEREXACT)).all():
-      raise NotImplementedError(f"actuator dynamics type(s) {sorted(set(dyn[~np.isin(dyn, (0, 1, 2, 3))].tolist()))} are not implemented (none, integrator, filter, filterexact are)")
+    if not np.isin(dyn, (C.DYN_NONE, C.DYN_INTEGRATOR, C.DYN_FILTER, C.DYN_FILTEREXACT, C.DYN_MUSCLE)).all():
+      raise NotImplementedError(f"actuator dynamics type(s) {sorted(set(dyn[~np.isin(dyn, (0, 1, 2, 3, 4))].tolist()))} are not implemented (none, integrator, filter, filterexact, muscle are)")
+    muscle = np.isin(gt, (C.GAIN_MUSCLE,)) | np.isin(bt, (C.BIAS_MUSCLE,))
+    if muscle.any():
+      # the muscle curves divide by the optimum length (lengthrange[1] - lengthrange[0]) / (range[1] - range[0]) (util_misc.py:500)
+      lr = np.asarray(getattr(mjm, "actuator_lengthrange", np.zeros((mjm.nu, 2))), dtype=np.float64).reshape(mjm.nu, 2)
+      bad = np.nonzero(muscle & ~(lr[:, 0] < lr[:, 1]))[0]
+      if len(bad):
+        raise ValueError(f"muscle actuator(s) {bad.tolist()}: actuator_lengthrange must satisfy lengthrange[0] < lengthrange[1] (got {lr[bad].tolist()})")
   for n in ("dof_dampingpoly", "jnt_stiffnesspoly"):
     if hasattr(mjm, n) and np.any(np.asarray(getattr(mjm, n)) != 0):
       raise NotImplementedError(f"{n}: polynomial stiffness / damping is not implemented")
@@ -524,8 +531,10 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   m.actuator_actlimited = dev_i(np.asarray(getattr(mjm, "actuator_actlimited", np.zeros(nu_))).astype(np.int32))
   m.actuator_actearly = dev_i(np.asarray(getattr(mjm, "actuator_actearly", np.zeros(nu_))).astype(np.int32))
   m.actuator_dynprm = dev_f(np.asarray(getattr(mjm, "actuator_dynprm", np.zeros((nu_, 10)))).reshape(nu_, 10), name="actuator_dynprm")
-  # acceleration of a unit actuator force at qpos0 (set_const.py:493-504); nothing in the step reads it (no muscles here)
+  # acceleration of a unit actuator force at qpos0 (set_const.py:493-504): the force scale of muscles with force < 0
   m.actuator_acc0 = dev_f(np.asarray(getattr(mjm, "actuator_acc0", np.zeros(nu_))).reshape(nu_), name="actuator_acc0")
+  # feasible length range (types.py:1315): the muscles' optimum length and normalized length (util_misc.py:481-558)
+  m.actuator_lengthrange = dev_f(np.asarray(getattr(mjm, "actuator_lengthrange", np.zeros((nu_, 2)))).reshape(nu_, 2), name="actuator_lengthrange")
   m.actuator_actrange = dev_f(np.asarray(getattr(mjm, "actuator_actrange", np.zeros((nu_, 2)))).reshape(nu_, 2), name="actuator_actrange")
   # fixed tendons (smooth.py:3658; constraint.py:642, 1867, 2243; passive.py:208): path, Jacobian sparsity and constant entries
   nt = int(getattr(mjm, "ntendon", 0))
@@ -695,7 +704,7 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
                                          "ten_J_rownnz", "ten_J_rowadr", "ten_J_colind", "tendon_adr", "tendon_num", "wrap_objid", "tendon_limited", "tendon_actfrclimited", "wrap_prm", "ten_J0",
                                          "geom_group", "geom_matid", "geom_rgba", "mat_rgba", "mesh_faceadr", "mesh_face",
                                          "geom_fluid", "body_fluid", "body_geomadr", "body_geomnum", "sensor_collision_start_adr", "sensor_collision_pair",
-                                         "sensor_collision_id", "sensor_collision_adr", "sensor_collision_flip", "actuator_acc0", "sensor_energy_adr",
+                                         "sensor_collision_id", "sensor_collision_adr", "sensor_collision_flip", "actuator_acc0", "actuator_lengthrange", "jnt_limited", "sensor_energy_adr",
                                          "actuator_history", "actuator_historyadr", "actuator_delay", "sensor_history", "sensor_historyadr", "sensor_delay",
                                          "sensor_interval", "sensor_history_id"]
                                         + [n for n, _ in _TENDON_FLOATS]):

@@ -288,6 +288,8 @@ def _geom_aabb(gtype, size):
 # ----------------------------------------------------------------------------------------------
 
 _ACT_TAGS = ("general", "motor", "position", "velocity", "intvelocity", "damper", "cylinder", "muscle", "adhesion")
+# the <muscle> shortcut's scalar parameters after range, in gainprm / biasprm order, with MuJoCo's defaults
+_MUSCLE_DEFAULTS = (("force", -1.0), ("scale", 200.0), ("lmin", 0.5), ("lmax", 1.6), ("vmax", 1.5), ("fpmax", 1.3), ("fvmax", 1.2))
 # delay / history attributes of actuators and sensors; interp keywords as in the reference's history.py:88 (0 zoh, 1 linear, 2 cubic)
 _HISTORY_KEYS = ("nsample", "interp", "delay", "interval")
 _INTERP = {"zoh": 0, "linear": 1, "cubic": 2}
@@ -1274,7 +1276,10 @@ def compile_xml(root):
   m.names.actuator = []
   m.actuator_history = np.zeros((nu, 2), dtype=np.int32)
   m.actuator_delay = np.zeros(nu)
-  dyn_names = {"none": C.DYN_NONE, "integrator": C.DYN_INTEGRATOR, "filter": C.DYN_FILTER, "filterexact": C.DYN_FILTEREXACT}
+  m.actuator_lengthrange = np.zeros((nu, 2))
+  dyn_names = {"none": C.DYN_NONE, "integrator": C.DYN_INTEGRATOR, "filter": C.DYN_FILTER, "filterexact": C.DYN_FILTEREXACT, "muscle": C.DYN_MUSCLE}
+  gain_names = {"fixed": C.GAIN_FIXED, "affine": C.GAIN_AFFINE, "muscle": C.GAIN_MUSCLE}
+  bias_names = {"none": C.BIAS_NONE, "affine": C.BIAS_AFFINE, "muscle": C.BIAS_MUSCLE}
   for i, (tag, a) in enumerate(acts):
     m.names.actuator.append(a.get("name", f"actuator{i}"))
     m.actuator_history[i], m.actuator_delay[i], _ = _history_attrs(a, f"actuator '{m.names.actuator[-1]}'", interval=False)
@@ -1293,14 +1298,19 @@ def compile_xml(root):
     if tag == "general":
       dyn = a.get("dyntype", "none")
       if dyn not in dyn_names:
-        raise NotImplementedError(f"actuator dyntype '{dyn}' is not supported (none, integrator, filter, filterexact are)")
+        raise NotImplementedError(f"actuator dyntype '{dyn}' is not supported (none, integrator, filter, filterexact, muscle are)")
       m.actuator_dyntype[i] = dyn_names[dyn]
       if "dynprm" in a:
         dp = _vec(a["dynprm"])
         m.actuator_dynprm[i, :] = 0
         m.actuator_dynprm[i, : dp.size] = dp
-      m.actuator_gaintype[i] = {"fixed": C.GAIN_FIXED, "affine": C.GAIN_AFFINE}[a.get("gaintype", "fixed")]
-      m.actuator_biastype[i] = {"none": C.BIAS_NONE, "affine": C.BIAS_AFFINE}[a.get("biastype", "none")]
+      gt, bt = a.get("gaintype", "fixed"), a.get("biastype", "none")
+      if gt not in gain_names:
+        raise NotImplementedError(f"actuator gaintype '{gt}' is not supported (fixed, affine, muscle are)")
+      if bt not in bias_names:
+        raise NotImplementedError(f"actuator biastype '{bt}' is not supported (none, affine, muscle are)")
+      m.actuator_gaintype[i] = gain_names[gt]
+      m.actuator_biastype[i] = bias_names[bt]
       if "gainprm" in a:
         gp = _vec(a["gainprm"])
         m.actuator_gainprm[i, :] = 0
@@ -1347,8 +1357,20 @@ def compile_xml(root):
       m.actuator_gainprm[i, 0] = kv
       m.actuator_biastype[i] = C.BIAS_AFFINE
       m.actuator_biasprm[i, 2] = -kv
+    elif tag == "muscle":  # MuJoCo's <muscle> shortcut: dynprm = (timeconst, tausmooth), gainprm = biasprm = the 9 muscle parameters
+      m.actuator_dyntype[i], m.actuator_gaintype[i], m.actuator_biastype[i] = C.DYN_MUSCLE, C.GAIN_MUSCLE, C.BIAS_MUSCLE
+      m.actuator_dynprm[i, :] = 0
+      m.actuator_dynprm[i, :2] = _vec(a.get("timeconst"), 2, default=[0.01, 0.04])
+      m.actuator_dynprm[i, 2] = float(a.get("tausmooth", 0.0))
+      m.actuator_gainprm[i, :] = 0
+      m.actuator_gainprm[i, :2] = _vec(a.get("range"), 2, default=[0.75, 1.05])
+      for k, (key, val) in enumerate(_MUSCLE_DEFAULTS):
+        m.actuator_gainprm[i, 2 + k] = float(a.get(key, val))
+      m.actuator_biasprm[i, :] = m.actuator_gainprm[i]
     else:
       raise NotImplementedError(f"actuator shortcut <{tag}> is not supported")
+    if "lengthrange" in a:
+      m.actuator_lengthrange[i] = _vec(a["lengthrange"], 2)
     m.actuator_actearly[i] = a.get("actearly", "false") == "true"
     if m.actuator_dyntype[i] != C.DYN_NONE or int(a.get("actdim", -1)) > 0:
       m.actuator_actnum[i] = int(a.get("actdim", -1)) if int(a.get("actdim", -1)) > 0 else 1
@@ -1359,6 +1381,8 @@ def compile_xml(root):
         getattr(m, "actuator_" + rng)[i] = _vec(a[rng])
       l = a.get(lim, "auto")
       getattr(m, "actuator_" + lim)[i] = (l == "true") or (l == "auto" and compiler["autolimits"] and rng in a)
+
+  _set_length_range(m, [tag for tag, _ in acts], ["lengthrange" in a for _, a in acts])
 
   # ---- contact excludes / pairs
   excl, pairs = [], []
@@ -1725,6 +1749,37 @@ def _tendon_row(m, t):
   for k in range(m.tendon_adr[t], m.tendon_adr[t] + m.tendon_num[t]):
     J[m.jnt_dofadr[m.wrap_objid[k]]] += m.wrap_prm[k]
   return J
+
+
+def _set_length_range(m, tags, explicit):
+  """actuator_lengthrange: an explicit `lengthrange` is kept; otherwise a muscle on a limited joint or limited fixed tendon gets the
+  limit range times gear[0], ends swapped for a negative gear (the rule of the reference's set_const.py:573-607; MuJoCo's compiler
+  finds the range by simulation instead).  Any other actuator keeps (0, 0).  A muscle with neither is refused by name."""
+  for i in range(m.nu):
+    muscle = m.actuator_gaintype[i] == C.GAIN_MUSCLE or m.actuator_biastype[i] == C.BIAS_MUSCLE
+    if not muscle:
+      continue
+    if explicit[i]:
+      _check_muscle_lengthrange(m, i, tags[i])
+      continue
+    j, gear = int(m.actuator_trnid[i, 0]), float(m.actuator_gear[i, 0])
+    if m.actuator_trntype[i] == C.TRN_JOINT and m.jnt_limited[j]:
+      rng = m.jnt_range[j]
+    elif m.actuator_trntype[i] == C.TRN_TENDON and m.tendon_limited[j]:
+      rng = m.tendon_range[j]
+    else:
+      raise NotImplementedError(f"muscle actuator '{m.names.actuator[i]}' ({tags[i]}) needs a lengthrange: give lengthrange= or put it on a limited "
+                                "joint or tendon (the simulation-based lengthrange computation is not implemented)")
+    m.actuator_lengthrange[i] = (rng[0] * gear, rng[1] * gear) if gear > 0 else (rng[1] * gear, rng[0] * gear)
+    _check_muscle_lengthrange(m, i, tags[i])
+
+
+def _check_muscle_lengthrange(m, i, tag):
+  """A muscle's optimum length is (lengthrange[1] - lengthrange[0]) / (range[1] - range[0]): an empty or reversed lengthrange (equal
+  limits, gear 0, or an explicit range given backwards) would divide by MJ_MINVAL in the muscle curves."""
+  lo, hi = m.actuator_lengthrange[i]
+  if not lo < hi:
+    raise ValueError(f"muscle actuator '{m.names.actuator[i]}' ({tag}): lengthrange must satisfy lengthrange[0] < lengthrange[1], got ({lo}, {hi})")
 
 
 def _set_const(m):

@@ -78,3 +78,22 @@ def set_const(m: Model, d: Data, restore: bool = True):
   """set_const_fixed, set_const_0 and set_const_spring, then (with `restore`) the position stages and the factor of M at d.qpos
   (set_const.py:881).  Call it after changing body masses, inertias, qpos0, qpos_spring, armature, eq_data or dampratio actuators."""
   _set_const(m, d, FIXED | ZERO | SPRING, restore)
+
+
+def set_length_range(m: Model, d: Data, index: int = -1):
+  """actuator_lengthrange from the joint and tendon limits (set_const.py:952): an actuator on a limited joint or limited fixed tendon
+  gets the limit range times gear[0], ends swapped for a negative gear; every other actuator gets (0, 0).  As in the reference, every
+  actuator is computed whatever `index` is (-1 or an actuator id).  Entry i of a batched `m.actuator_lengthrange` is computed from
+  world i; call it after changing `jnt_range`, `tendon_range` or `actuator_gear` of a model with muscles."""
+  if not isinstance(m, Model) or not isinstance(d, Data):
+    raise TypeError(f"expected (Model, Data), got ({type(m).__name__}, {type(d).__name__})")
+  if d._model is not m and d._model._handle != m._handle:
+    raise ValueError("Data was created for a different Model")
+  if not -1 <= int(index) < m.nu:
+    raise ValueError(f"index must be -1 or an actuator id in [0, {m.nu}), got {index}")
+  if m.nu == 0:
+    return
+  n = int(m.actuator_lengthrange.shape[0])
+  if n > d.nworld:
+    raise ValueError(f"Model.actuator_lengthrange has {n} per-world entries but Data has {d.nworld} worlds: entry i is computed from world i")
+  _lib.check(_lib.lib().mjb_set_length_range(m._handle, d._handle, int(index), torch.cuda.current_stream().cuda_stream))

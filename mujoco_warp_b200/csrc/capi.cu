@@ -120,7 +120,8 @@ int mjb_model_set_array_batched(mjbModel* m, const char* name, const void* p, in
   MJB_HISTORY_IARRS(X)
   MJB_HISTORY_FARRS(X)
 #undef X
-  if (!strcmp(name, "actuator_acc0")) { m->setc.actuator_acc0 = (float*)p; m->setc.nb_actuator_acc0 = nbatch; return 0; }
+  // set_const writes actuator_acc0 through SetConstDev; the muscle actuators read it through ModelDev (below)
+  if (!strcmp(name, "actuator_acc0")) { m->setc.actuator_acc0 = (float*)p; m->setc.nb_actuator_acc0 = nbatch; }
   if (!strcmp(name, "meaninertia")) {
     if (nbatch != 1) return fail("meaninertia is a Model scalar (not batched)");
     m->setc.meaninertia = (float*)p;
@@ -585,6 +586,16 @@ int mjb_set_const(const mjbModel* m, mjbData* d, int parts, int restore, void* s
     MJB_LAUNCH(launch_position(md, d->dev, STG_KINEMATICS | STG_COM_POS | STG_CAMLIGHT | STG_CRB | STG_TRANSMISSION, s));
     MJB_LAUNCH(launch_velocity(md, d->dev, STG_FACTOR_ONLY, s, fluid(m, d)));
   }
+  return 0;
+}
+
+int mjb_set_length_range(const mjbModel* m, mjbData* d, int index, void* stream) {
+  MJB_ENTER();
+  const ModelDev& md = m->dev;
+  if (index < -1 || index >= md.nu) return fail("mjb_set_length_range: index must be -1 or an actuator id in [0, " + std::to_string(md.nu) + "), got " + std::to_string(index));
+  const int nb = md.nb_actuator_lengthrange, nworld = d->dev.nworld;
+  if (nb > nworld) return fail("mjb_set_length_range: Model.actuator_lengthrange has " + std::to_string(nb) + " entries, more than the Data's " + std::to_string(nworld) + " worlds");
+  MJB_LAUNCH(launch_set_length_range(md, nb, nworld, s));
   return 0;
 }
 

@@ -1,6 +1,7 @@
 // k_set_const.cu -- recomputes the Model constants the compiler derives from other Model fields, per world.
 //
-// Replaces (reference, /root/reference/mujoco_warp/_src/): set_const.py:613 set_const_fixed, :634 set_const_0, :847 set_const_spring.
+// Replaces (reference, /root/reference/mujoco_warp/_src/): set_const.py:613 set_const_fixed, :634 set_const_0, :847 set_const_spring,
+// :952 set_length_range.
 // The reference runs one solve_m launch (plus helpers) per dof, per body x 6 Jacobian rows, per tendon and per actuator.  Here one
 // warp per world solves all of these right-hand sides against the factor the world already holds (Data.qLD, per-tree dense upper U
 // with M = U^T U, k_support.cu): U is staged in shared memory once, the lanes take one right-hand side each, so every factor read is
@@ -23,6 +24,29 @@ __global__ void k_set_const_fixed(const __grid_constant__ ModelDev mp, int nw, i
   float* sub = const_cast<float*>(m.body_subtreemass);
   for (int b = 0; b < m.nbody; b++) sub[b] = m.body_mass[b];
   for (int b = m.nbody - 1; b > 0; b--) sub[m.body_parentid[b]] += sub[b];
+}
+
+// ---------------------------------------------------------------- set_length_range (set_const.py:573-607, 952-985)
+// One thread per (world, actuator) of worlds [0, nw): the range of a limited joint or fixed tendon times gear[0] (ends swapped for a
+// negative gear), (0, 0) for any other transmission.  Every actuator is written, muscle or not, as the reference does.
+__global__ void k_set_length_range(const __grid_constant__ ModelDev mp, int nw, int nworld) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= nw * mp.nu) return;
+  const int w = i / mp.nu, a = i - w * mp.nu;
+  const ModelDev m = world_model(mp, w, nworld);
+  const int trn = m.actuator_trntype[a], id = m.actuator_trnid[2 * a];
+  const float gear = m.actuator_gear[6 * a];
+  const float* rng = nullptr;
+  if (trn == TRN_JOINT && m.jnt_limited[id]) rng = m.jnt_range + 2 * id;
+  else if (trn == TRN_TENDON && m.ntendon > 0 && m.tendon_limited[id]) rng = m.tendon_range + 2 * id;
+  float lo = 0.f, hi = 0.f;
+  if (rng) {
+    if (gear > 0.f) { lo = rng[0] * gear; hi = rng[1] * gear; }
+    else { lo = rng[1] * gear; hi = rng[0] * gear; }
+  }
+  float* out = const_cast<float*>(m.actuator_lengthrange) + 2 * a;
+  out[0] = lo;
+  out[1] = hi;
 }
 
 // ---------------------------------------------------------------- qpos swap (set_const.py:59-66, 656-658, 833)
@@ -269,6 +293,11 @@ size_t smem_set_const(const ModelDev& m) { return sizeof(float) * set_const_word
 
 cudaError_t launch_set_const_fixed(const ModelDev& m, int nw, int nworld, cudaStream_t s) {
   return launch(k_set_const_fixed, (nw + 127) / 128, 128, 0, s, m, nw, nworld);
+}
+cudaError_t launch_set_length_range(const ModelDev& m, int nw, int nworld, cudaStream_t s) {
+  const int n = nw * m.nu;
+  if (n == 0) return cudaSuccess;
+  return launch(k_set_length_range, (n + 127) / 128, 128, 0, s, m, nw, nworld);
 }
 cudaError_t launch_set_const_qpos(const ModelDev& m, const DataDev& d, const SetConstDev& c, int mode, int nw, cudaStream_t s) {
   const int n = nw * m.nq;

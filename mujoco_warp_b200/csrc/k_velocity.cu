@@ -13,6 +13,7 @@
 
 #include "mjb_fluid.cuh"
 #include "mjb_math.cuh"
+#include "mjb_muscle.cuh"
 #include "mjb_team.cuh"
 #include "mjb_types.cuh"
 

@@ -283,14 +283,19 @@
         float gain = 0.f, bias = 0.f;
         if (m.actuator_gaintype[a] == GAIN_FIXED) gain = gp[0];
         else if (m.actuator_gaintype[a] == GAIN_AFFINE) gain = gp[0] + gp[1] * length + gp[2] * velocity;
+        else if (m.actuator_gaintype[a] == GAIN_MUSCLE)  // forward.py:976-980, per-world acc0 and lengthrange
+          gain = muscle_gain(length, velocity, m.actuator_lengthrange[2 * a], m.actuator_lengthrange[2 * a + 1], m.actuator_acc0[a], gp);
         if (m.actuator_biastype[a] == BIAS_AFFINE) bias = bp[0] + bp[1] * length + bp[2] * velocity;
+        else if (m.actuator_biastype[a] == BIAS_MUSCLE)  // forward.py:1016-1019
+          bias = muscle_bias(length, m.actuator_lengthrange[2 * a], m.actuator_lengthrange[2 * a + 1], m.actuator_acc0[a], bp);
         float ctrl_act = ctrl;
-        if (m.na > 0 && m.actuator_actadr[a] >= 0) {  // stateful actuator (forward.py:800-963): INTEGRATOR / FILTER / FILTEREXACT
+        if (m.na > 0 && m.actuator_actadr[a] >= 0) {  // stateful actuator (forward.py:800-963): INTEGRATOR / FILTER / FILTEREXACT / MUSCLE
           const int last = m.actuator_actadr[a] + m.actuator_actnum[a] - 1, dyn = m.actuator_dyntype[a];
           const float act = d.act[wb * m.na + last];
           float act_dot = 0.f;
           if (dyn == DYN_INTEGRATOR) act_dot = ctrl;
           else if (dyn == DYN_FILTER || dyn == DYN_FILTEREXACT) act_dot = (ctrl - act) / fmaxf(m.actuator_dynprm[10 * a], MJ_MINVAL);
+          else if (dyn == DYN_MUSCLE) act_dot = muscle_dynamics(ctrl, act, m.actuator_dynprm + 10 * a);
           if (valid) d.act_dot[wb * m.na + last] = act_dot;
           ctrl_act = m.actuator_actearly[a] ? next_act(m, a, act, act_dot, 1.0f, m.actuator_actlimited[a] != 0) : act;
         }

@@ -26,7 +26,7 @@
   X(nxn_geom_pair) X(nxn_pairid) X(body_isdofancestor) X(eq_type) X(eq_obj1id) X(eq_obj2id) X(jnt_limited_ball_adr) X(pair_dim) \
   X(sensor_type) X(sensor_datatype) X(sensor_needstage) X(sensor_objtype) X(sensor_objid) X(sensor_reftype) X(sensor_refid) X(sensor_dim) X(sensor_adr) X(site_type) \
   X(geom_dataid) X(mesh_vertadr) X(mesh_vertnum) X(mesh_graphadr) X(mesh_graph) X(mesh_polynum) X(mesh_polyadr) X(mesh_polyvertadr) X(mesh_polyvertnum) \
-  X(mesh_polyvert) X(mesh_polymapadr) X(mesh_polymapnum) X(mesh_polymap) X(geom_group) X(geom_matid) X(mesh_faceadr) X(mesh_face)
+  X(mesh_polyvert) X(mesh_polymapadr) X(mesh_polymapnum) X(mesh_polymap) X(geom_group) X(geom_matid) X(mesh_faceadr) X(mesh_face) X(jnt_limited)
 #define MJB_MODEL_FARRS(X) \
   X(qpos0) X(qpos_spring) X(body_pos) X(body_quat) X(body_ipos) X(body_iquat) X(body_mass) X(body_subtreemass) \
   X(body_inertia) X(body_invweight0) X(body_gravcomp) X(jnt_pos) X(jnt_axis) X(jnt_stiffness) X(jnt_range) X(jnt_margin) X(jnt_solref) \
@@ -39,7 +39,7 @@
   X(sensor_cutoff) X(site_size) X(mesh_vert) X(mesh_polynormal) X(actuator_dynprm) X(actuator_actrange) \
   X(wrap_prm) X(ten_J0) X(tendon_range) X(tendon_margin) X(tendon_stiffness) X(tendon_damping) X(tendon_frictionloss) X(tendon_lengthspring) \
   X(tendon_length0) X(tendon_invweight0) X(tendon_solref_lim) X(tendon_solimp_lim) X(tendon_solref_fri) X(tendon_solimp_fri) X(tendon_actfrcrange) \
-  X(geom_rgba) X(mat_rgba)
+  X(geom_rgba) X(mat_rgba) X(actuator_acc0) X(actuator_lengthrange)
 
 struct ModelDev {
 #define X(n) int n;
@@ -211,9 +211,9 @@ enum { SENS_TOUCH = 0, SENS_ACCELEROMETER = 1, SENS_VELOCIMETER = 2, SENS_GYRO =
 enum { CNSTR_EQUALITY = 0, CNSTR_FRICTION_DOF = 1, CNSTR_FRICTION_TENDON = 2, CNSTR_LIMIT_JOINT = 3, CNSTR_LIMIT_TENDON = 4, CNSTR_CONTACT_FRICTIONLESS = 5, CNSTR_CONTACT_PYRAMIDAL = 6, CNSTR_CONTACT_ELLIPTIC = 7 };
 enum { ST_SATISFIED = 0, ST_QUADRATIC = 1, ST_LINEARNEG = 2, ST_LINEARPOS = 3, ST_CONE = 4 };
 enum { CAM_FIXED = 0, CAM_TRACK, CAM_TRACKCOM, CAM_TARGETBODY, CAM_TARGETBODYCOM };
-enum { GAIN_FIXED = 0, GAIN_AFFINE = 1 };
-enum { DYN_NONE = 0, DYN_INTEGRATOR = 1, DYN_FILTER = 2, DYN_FILTEREXACT = 3 };
-enum { BIAS_NONE = 0, BIAS_AFFINE = 1 };
+enum { GAIN_FIXED = 0, GAIN_AFFINE = 1, GAIN_MUSCLE = 2 };
+enum { DYN_NONE = 0, DYN_INTEGRATOR = 1, DYN_FILTER = 2, DYN_FILTEREXACT = 3, DYN_MUSCLE = 4 };
+enum { BIAS_NONE = 0, BIAS_AFFINE = 1, BIAS_MUSCLE = 2 };
 enum {
   DSBL_CONSTRAINT = 1 << 0, DSBL_EQUALITY = 1 << 1, DSBL_FRICTIONLOSS = 1 << 2, DSBL_LIMIT = 1 << 3, DSBL_CONTACT = 1 << 4,
   DSBL_SPRING = 1 << 5, DSBL_DAMPER = 1 << 6, DSBL_GRAVITY = 1 << 7, DSBL_CLAMPCTRL = 1 << 8, DSBL_WARMSTART = 1 << 9,
@@ -280,6 +280,8 @@ cudaError_t launch_set_const_qpos(const ModelDev& m, const DataDev& d, const Set
 cudaError_t launch_set_const_0(const ModelDev& m, const DataDev& d, const SetConstDev& c, int nw, cudaStream_t s);
 cudaError_t launch_set_const_spring(const ModelDev& m, const DataDev& d, int nw, cudaStream_t s);
 size_t smem_set_const(const ModelDev& m);
+// set_length_range (k_set_const.cu): actuator_lengthrange of worlds [0, nw) from the joint / tendon limits and gear
+cudaError_t launch_set_length_range(const ModelDev& m, int nw, int nworld, cudaStream_t s);
 // energy (k_energy.cu): the ENERGY_* parts of d's world range
 cudaError_t launch_energy(const ModelDev& m, const DataDev& d, const EnergyDev& e, int parts, cudaStream_t s);
 size_t smem_integrate(const ModelDev& m);
