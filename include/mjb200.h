@@ -34,6 +34,10 @@
  *   mjb_contact_force          <- _src/support.py:445  contact_force(m, d, contact_ids, to_world_frame, force)
  *   mjb_rays                   <- _src/ray.py:1219 rays(m, d, pnt, vec, geomgroup, flg_static, bodyexclude, dist, geomid, normal) without a
  *                                 render context (every geom tested, no BVH; no height fields)
+ *   mjb_refit_bvh              <- _src/bvh.py:39 refit_bvh(m, d, rc): world-space bounds of the rendered geoms (no BVH is built;
+ *                                 the renderer culls every geom against its bounds)
+ *   mjb_render                 <- _src/render.py:656 render(m, d, rc) without textures, skybox, splats or flex
+ *   mjb_render_rays            <- _src/render_util.py:255 _build_rays (the precomputed rays of create_render_context)
  *   mjb_rungekutta4            <- _src/forward.py:523  rungekutta4(m, d)
  *   mjb_solve                  <- _src/solver.py:3671  solve
  *   mjb_euler                  <- _src/forward.py:387  euler (always the semi-implicit Euler update, whatever the model's integrator)
@@ -141,6 +145,66 @@ int mjb_contact_force(const mjbModel* m, mjbData* d, const int* contact_ids, int
  * lowest geom id wins.  One kernel launch (none for nray = 0). */
 int mjb_rays(const mjbModel* m, mjbData* d, const float* pnt, const float* vec, int nray, int pnt_nbatch, const int* geomgroup,
              int flg_static, const int* bodyexclude, float* dist, int* geomid, float* normal, void* stream);
+/* The render context of mjb_refit_bvh / mjb_render (render_util.py:272 create_render_context; types.py RenderContext): the cameras
+ * that render, their pixel buffers and the enabled geoms, plus the Model's camera, light and material fields the renderer reads.  All
+ * pointers are device pointers.  A per-world Model field has nb_<field> entries (world w reads entry w % nb); 1 = shared. */
+typedef struct mjbRender {
+  int ncam;                      /* cameras that render (the context's active cameras) */
+  int ngeom;                     /* enabled geoms (geom group filter) */
+  int npixel;                    /* pixels of all active cameras */
+  int nrgb, ndepth, nseg;        /* row lengths of rgb / depth / seg (pixels of the cameras that render each output) */
+  const int* cam_id;             /* (ncam) Model camera id of each active camera */
+  const int* cam_res;            /* (ncam, 2) width, height */
+  const int* pix_adr;            /* (ncam) first pixel of each camera in the ray table */
+  const int* rgb_adr;            /* (ncam) first pixel in rgb, -1: not rendered; depth_adr / seg_adr likewise */
+  const int* depth_adr;
+  const int* seg_adr;
+  const float* ray;              /* (npixel, 3) camera-frame ray directions (use_precomputed_rays), else NULL */
+  const int* geom_id;            /* (ngeom) enabled geom ids, ascending */
+  const float* mesh_half;        /* (nmesh, 3) half-extent of each mesh's vertex box (the bounds of its geoms) */
+  float* lower;                  /* (nworld, ngeom, 3) world-space bounds written by mjb_refit_bvh */
+  float* upper;
+  unsigned* rgb;                 /* (nworld, nrgb) packed 0xAARRGGBB */
+  float* depth;                  /* (nworld, ndepth) planar depth */
+  int* seg;                      /* (nworld, nseg, 2) geom id, object type */
+  const int* cam_projection;     /* (ncam_model) */
+  const float* cam_fovy;         /* (nb, ncam_model) */
+  const float* cam_sensorsize;   /* (ncam_model, 2) */
+  const float* cam_intrinsic;    /* (nb, ncam_model, 4) */
+  int nb_cam_fovy, nb_cam_intrinsic;
+  int nlight;
+  const int* light_type;         /* (nlight) */
+  const int* light_castshadow;
+  const int* light_active;
+  const float* light_attenuation; /* (nb, nlight, 3) */
+  const float* light_cutoff;     /* (nb, nlight) degrees */
+  const float* light_exponent;
+  const float* light_ambient;    /* (nb, nlight, 3) */
+  const float* light_diffuse;
+  const float* light_specular;
+  int nb_light_attenuation, nb_light_cutoff, nb_light_exponent, nb_light_ambient, nb_light_diffuse, nb_light_specular;
+  const float* mat_specular;     /* (nb, nmat) */
+  const float* mat_shininess;
+  const float* mat_emission;
+  int nb_mat_specular, nb_mat_shininess, nb_mat_emission;
+  int use_shadows, use_ambient_lighting, enable_per_light_ambient, enable_specular, enable_emission, enable_backface_culling;
+  int headlight_active, light_attenuation_is_default, has_spot_lights;
+  unsigned background_color;     /* packed like rgb */
+  float znear;
+  float headlight_ambient[3], headlight_diffuse[3], headlight_specular[3];
+} mjbRender;
+/* render_util.py:255 _build_rays (create_render_context with use_precomputed_rays): ray (npixel, 3) receives the camera-frame ray of
+ * every pixel of rc's active cameras, from entry 0 of cam_fovy / cam_intrinsic.  Needs rc's camera tables only.  One kernel launch. */
+int mjb_render_rays(const mjbRender* rc, float* ray, void* stream);
+/* bvh.py:39 refit_bvh: lower / upper of every enabled geom of every world from d.geom_xpos / geom_xmat (bvh.py:178 _compute_bvh_bounds,
+ * with its 1000-unit extent for infinite planes).  One kernel launch. */
+int mjb_refit_bvh(const mjbModel* m, mjbData* d, const mjbRender* rc, void* stream);
+/* render.py:656 render: one image per (world, active camera) into rc's rgb / depth / seg.  Reads geom_xpos / geom_xmat, cam_xpos /
+ * cam_xmat and light_xpos / light_xdir of the last kinematics and the bounds of the last mjb_refit_bvh; writes no Data field.  Each pixel
+ * casts its primary ray against every enabled geom whose bounds it enters (closest hit; equal distances go to the lower geom id), shades
+ * it with emission, ambient, every light's diffuse / specular term and the headlight, and with use_shadows casts a shadow ray per light.
+ * A miss writes background_color, depth 0 and (-1, -1).  One kernel launch. */
+int mjb_render(const mjbModel* m, mjbData* d, const mjbRender* rc, void* stream);
 /* forward.py:523 rungekutta4(m, d): the integrator alone, after forward() (models compiled with the RK4 integrator) */
 int mjb_rungekutta4(const mjbModel* m, mjbData* d, void* stream);
 int mjb_solve(const mjbModel* m, mjbData* d, void* stream);

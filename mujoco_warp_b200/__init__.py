@@ -3,7 +3,8 @@
 Public surface mirrors /root/reference/mujoco_warp/__init__.py for the step path: put_model, put_data, make_data,
 reset_data, step, forward, the individually callable stages, potential and kinetic energy (energy_pos / energy_vel), actuator and sensor
 delays (read_ctrl / read_sensor / init_ctrl_history / init_sensor_history), inverse
-dynamics (inverse), ray casting (ray / rays) and the per-world recomputation of derived Model constants (set_const, set_const_fixed, set_const_0, set_const_spring,
+dynamics (inverse), ray casting (ray / rays), batch rendering (create_render_context, refit_bvh, render, get_rgb / get_depth /
+get_segmentation) and the per-world recomputation of derived Model constants (set_const, set_const_fixed, set_const_0, set_const_spring,
 set_length_range); `mjcf.load` stands in for mujoco's MJCF compiler.
 """
 
@@ -17,11 +18,12 @@ from ._src.forward import com_vel, contact_force, fwd_kinematics, get_state, imp
 from ._src.history import init_ctrl_history, init_sensor_history, read_ctrl, read_sensor
 from ._src.inverse import inverse
 from ._src.ray import ray, rays
+from ._src.render import create_render_context, get_depth, get_rgb, get_segmentation, refit_bvh, render
 from ._src.set_const import set_const, set_const_0, set_const_fixed, set_const_spring, set_length_range
 from ._src.io import get_data_into, load_trajectory, make_data, override_model, put_data, put_model, reset_data, reset_data_keyframe
 from ._src.trace import event_trace_step, flatten_trace
 from ._src.types import BroadphaseFilter, BroadphaseType, ConeType, Constraint, ConstraintState, ConstraintType, Contact, Data
 from ._src.types import BiasType, DynType, GainType, State, Statistic, TrnType
-from ._src.types import DisableBit, EnableBit, GeomType, IntegratorType, JointType, Model, Option, OverflowType, SolverType
+from ._src.types import DisableBit, EnableBit, GeomType, IntegratorType, JointType, Model, Option, OverflowType, RenderContext, SolverType
 
 __all__ = [n for n in dir() if not n.startswith("_")]

@@ -15,7 +15,7 @@ _PKG = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 _CSRC = os.path.join(_PKG, "csrc")
 LIB_PATH = os.environ.get("MJB_LIB", os.path.join(_PKG, "libmjb200.so"))  # MJB_LIB: A/B-test an alternative build
 HEADER_PATH = os.path.join(os.path.dirname(_PKG), "include", "mjb200.h")
-SOURCES = ["capi.cu", "k_position.cu", "k_collision.cu", "k_collision_mesh.cu", "k_constraint.cu", "k_velocity.cu", "k_solver.cu", "k_integrate.cu", "k_implicit.cu", "k_support.cu", "k_sensor.cu", "k_sensor_collision.cu", "k_ray.cu", "k_inverse.cu", "k_set_const.cu", "k_energy.cu", "k_history.cu"]
+SOURCES = ["capi.cu", "k_position.cu", "k_collision.cu", "k_collision_mesh.cu", "k_constraint.cu", "k_velocity.cu", "k_solver.cu", "k_integrate.cu", "k_implicit.cu", "k_support.cu", "k_sensor.cu", "k_sensor_collision.cu", "k_ray.cu", "k_inverse.cu", "k_set_const.cu", "k_energy.cu", "k_history.cu", "k_render.cu"]
 NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a", "--extended-lambda", "-Xcompiler", "-fPIC", "-shared"]
 
 _lib = None
@@ -112,6 +112,11 @@ def lib():
   L.mjb_contact_force.restype = ci
   L.mjb_rays.argtypes = [vp, vp, vp, vp, ci, ci, ctypes.POINTER(ci), ci, vp, vp, vp, vp, vp]
   L.mjb_rays.restype = ci
+  for f in ("mjb_refit_bvh", "mjb_render"):
+    getattr(L, f).argtypes = [vp, vp, vp, vp]
+    getattr(L, f).restype = ci
+  L.mjb_render_rays.argtypes = [vp, vp, vp]
+  L.mjb_render_rays.restype = ci
   L.mjb_set_const.argtypes = [vp, vp, ci, ci, vp]
   L.mjb_set_const.restype = ci
   L.mjb_set_length_range.argtypes = [vp, vp, ci, vp]

@@ -43,6 +43,9 @@ _TENDON_FLOATS = (("tendon_range", 2), ("tendon_margin", 1), ("tendon_stiffness"
 # float fields outside _FLOAT_FIELDS that carry the reference's `*` leading dimension as well
 _BATCHABLE_EXTRA = ("eq_solref", "eq_solimp", "eq_data", "pair_friction", "pair_solref", "pair_solreffriction", "pair_solimp", "pair_margin", "pair_gap",
                     "actuator_dynprm", "actuator_actrange", "geom_rgba", "mat_rgba", "actuator_acc0", "actuator_lengthrange") + tuple(n for n, _ in _TENDON_FLOATS)
+# the renderer's float Model fields that carry the reference's `*` leading dimension (types.py cam_fovy ... mat_emission)
+_RENDER_FLOATS = ("cam_fovy", "cam_intrinsic", "light_attenuation", "light_cutoff", "light_exponent", "light_ambient", "light_diffuse", "light_specular",
+                  "mat_specular", "mat_shininess", "mat_emission")
 _SIZES = ["nq", "nv", "nu", "na", "nbody", "njnt", "ngeom", "nsite", "ncam", "nlight", "ntree", "nkey", "nmocap", "neq", "ntendon", "nflex"]
 
 _SUPPORTED_PAIRS = {
@@ -444,6 +447,29 @@ def _validate_history(mjm):
         raise ValueError(f"{what}: {field} > 0 needs a history buffer (nsample > 0); with nsample = 0 it would be ignored")
 
 
+def render_fields(mjm) -> dict:
+  """The camera, light and material fields the renderer reads (MjModel names); models compiled before they existed get MuJoCo's
+  defaults (perspective 45-degree cameras of resolution 1 x 1 without a sensor, spot lights of diffuse 0.7 / specular 0.3 that cast
+  shadows, materials of specular 0.5 / shininess 0.5 without emission or texture).  mat_texid has MuJoCo's layout, one column per texture role."""
+  nc, nl, nm = int(getattr(mjm, "ncam", 0)), int(getattr(mjm, "nlight", 0)), int(getattr(mjm, "nmat", 0))
+
+  def g(name, n, shape, default, dt):
+    v = getattr(mjm, name, None)
+    return np.ascontiguousarray((np.broadcast_to(np.asarray(default), (n,) + shape) if v is None else np.asarray(v)).astype(dt).reshape((n,) + shape))
+
+  return dict(
+    cam_projection=g("cam_projection", nc, (), 0, np.int32), cam_fovy=g("cam_fovy", nc, (), 45.0, np.float64),
+    cam_resolution=g("cam_resolution", nc, (2,), 1, np.int32), cam_sensorsize=g("cam_sensorsize", nc, (2,), 0.0, np.float64),
+    cam_intrinsic=g("cam_intrinsic", nc, (4,), 0.0, np.float64),
+    light_type=g("light_type", nl, (), 0, np.int32), light_castshadow=g("light_castshadow", nl, (), 1, np.int32), light_active=g("light_active", nl, (), 1, np.int32),
+    light_attenuation=g("light_attenuation", nl, (3,), [1.0, 0.0, 0.0], np.float64), light_cutoff=g("light_cutoff", nl, (), 45.0, np.float64),
+    light_exponent=g("light_exponent", nl, (), 10.0, np.float64), light_ambient=g("light_ambient", nl, (3,), 0.0, np.float64),
+    light_diffuse=g("light_diffuse", nl, (3,), 0.7, np.float64), light_specular=g("light_specular", nl, (3,), 0.3, np.float64),
+    mat_specular=g("mat_specular", nm, (), 0.5, np.float64), mat_shininess=g("mat_shininess", nm, (), 0.5, np.float64), mat_emission=g("mat_emission", nm, (), 0.0, np.float64),
+    mat_texid=g("mat_texid", nm, (10,), -1, np.int32),  # (nmat, mjNTEXROLE)
+  )
+
+
 def _ptr_tensor(x: torch.Tensor) -> torch.Tensor:
   """A contiguous tensor with a valid device pointer (empty tables get a 1-element dummy)."""
   assert x.is_contiguous()
@@ -462,7 +488,7 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   for name, size in batch_sizes.items():
     if name in ("actuator_delay", "sensor_delay"):
       raise ValueError(f"Model field {name!r} is shared by all worlds (the reference has no per-world delays); it cannot be batched.")
-    if name not in _FLOAT_FIELDS and name not in _BATCHABLE_EXTRA:
+    if name not in _FLOAT_FIELDS and name not in _BATCHABLE_EXTRA and name not in _RENDER_FLOATS:
       raise ValueError(f"Model field {name!r} is not a batched array field.")
     if int(size) < 1:
       raise ValueError(f"batch_sizes[{name!r}] must be positive, got {size}.")
@@ -636,6 +662,9 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   m.geom_rgba = dev_f(np.asarray(getattr(mjm, "geom_rgba", np.tile([0.5, 0.5, 0.5, 1.0], (ng, 1)))).reshape(ng, 4), name="geom_rgba")
   m.nmat = int(getattr(mjm, "nmat", 0))
   m.mat_rgba = dev_f(np.asarray(mjm.mat_rgba).reshape(m.nmat, 4) if m.nmat else np.zeros((0, 4)), name="mat_rgba")
+  # the renderer's camera, light and material fields (render.py); read at each render() call, so they are not bound to the handle
+  for n, x in render_fields(mjm).items():
+    setattr(m, n, dev_f(x, name=n) if n in _RENDER_FLOATS else (dev_f(x, batched=False) if x.dtype == np.float64 else dev_i(x)))
   m.mesh_faceadr = dev_i(getattr(mjm, "mesh_faceadr", np.zeros(nmesh)) if nmesh else np.zeros(0))
   m.mesh_face = dev_i(np.asarray(getattr(mjm, "mesh_face", np.zeros((0, 3)))).reshape(-1, 3) if nmesh else np.zeros((0, 3)))
   m.nmeshface = int(m.mesh_face.shape[0])

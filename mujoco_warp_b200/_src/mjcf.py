@@ -326,6 +326,43 @@ def set_history_layout(m):
   m.actuator_historyadr, m.sensor_historyadr, m.nhistory = out["actuator"], out["sensor"], adr
 
 
+# The renderer's fields of <camera>, <light> and <visual><headlight>, with the defaults of MuJoCo's XML reference (not checked
+# against MuJoCo's own compiler, which is not available here).
+_CAMERA_FIELDS = (("projection", (), np.int32), ("fovy", (), np.float64), ("resolution", (2,), np.int32), ("sensorsize", (2,), np.float64), ("intrinsic", (4,), np.float64))
+_LIGHT_FIELDS = (("type", (), np.int32), ("castshadow", (), np.int32), ("active", (), np.int32), ("attenuation", (3,), np.float64), ("cutoff", (), np.float64),
+                 ("exponent", (), np.float64), ("ambient", (3,), np.float64), ("diffuse", (3,), np.float64), ("specular", (3,), np.float64))
+_TEX_ROLES = ("user", "rgb", "occlusion", "roughness", "metallic", "normal", "opacity", "emissive", "rgba", "orm")  # mjtTextureRole
+_LIGHT_TYPES = {"spot": 0, "directional": 1, "point": 2, "image": 3}
+_HEADLIGHT_DEFAULTS = (("active", 1), ("ambient", np.full(3, 0.1)), ("diffuse", np.full(3, 0.4)), ("specular", np.full(3, 0.5)))
+
+
+def _camera_optics(a):
+  """projection, fovy, resolution, sensorsize and intrinsic [fx, fy, cx, cy] (length units) of a resolved <camera>"""
+  ortho = a.get("projection", "orthographic" if a.get("orthographic") == "true" else "perspective")
+  if ortho not in ("perspective", "orthographic"):
+    raise ValueError(f"camera projection must be 'perspective' or 'orthographic', got {ortho!r}")
+  res = _vec(a.get("resolution"), 2, default=[1, 1])
+  sensor = _vec(a.get("sensorsize"), 2, default=[0, 0])
+  intr = np.concatenate([_vec(a.get("focal"), 2, default=[0, 0]), _vec(a.get("principal"), 2, default=[0, 0])])
+  fp, pp = _vec(a.get("focalpixel"), 2, default=[0, 0]), _vec(a.get("principalpixel"), 2, default=[0, 0])
+  if fp.any():
+    intr[:2] = fp / res * sensor
+  if pp.any():
+    intr[2:] = pp / res * sensor
+  return dict(projection=int(ortho == "orthographic"), fovy=float(a.get("fovy", 45.0)), resolution=res.astype(np.int32), sensorsize=sensor, intrinsic=intr)
+
+
+def _light_optics(a):
+  """type, castshadow, active, attenuation, cutoff, exponent and the ambient / diffuse / specular colours of a resolved <light>"""
+  kind = a.get("type", "directional" if a.get("directional") == "true" else "spot")
+  if kind not in _LIGHT_TYPES:
+    raise ValueError(f"light type must be one of {sorted(_LIGHT_TYPES)}, got {kind!r}")
+  return dict(type=_LIGHT_TYPES[kind], castshadow=int(a.get("castshadow", "true") == "true"), active=int(a.get("active", "true") == "true"),
+              attenuation=_vec(a.get("attenuation"), 3, default=[1, 0, 0]), cutoff=float(a.get("cutoff", 45.0)), exponent=float(a.get("exponent", 10.0)),
+              ambient=_vec(a.get("ambient"), 3, default=[0, 0, 0]), diffuse=_vec(a.get("diffuse"), 3, default=[0.7, 0.7, 0.7]),
+              specular=_vec(a.get("specular"), 3, default=[0.3, 0.3, 0.3]))
+
+
 class _Defaults:
   def __init__(self):
     self.classes = {"main": {}}
@@ -721,15 +758,24 @@ def compile_xml(root):
       meshes.append(_mesh.process(_vec(me.get("vertex")).reshape(-1, 3), None if ma.get("inertia") == "convex" else faces, _vec(ma.get("scale"), 3, default=[1, 1, 1])))
       mesh_names.append(me.get("name", f"mesh{len(mesh_names)}"))
 
-  # materials: only the colour is compiled (a fully transparent material hides its geoms from rays); every other material and
-  # texture attribute is ignored
-  mat_names, mat_rgba = [], []
+  # materials: the colour (a fully transparent material hides its geoms from rays) and the renderer's specular / shininess /
+  # emission, with MuJoCo's defaults.  A texture reference is only recorded (mat_texid): the renderer refuses textured materials.
+  tex_names = [te.get("name", f"texture{i}") for i, te in enumerate(e for asset in root.findall("asset") for e in asset.findall("texture"))]
+  mat_names, mat_rgba, mat_light = [], [], []
   for asset in root.findall("asset"):
     for me in asset.findall("material"):
       ma = dflt.resolve("material", me.get("class", "main"))
       ma.update(me.attrib)
       mat_names.append(me.get("name", f"material{len(mat_names)}"))
       mat_rgba.append(_vec(ma.get("rgba"), 4, default=[1, 1, 1, 1]))
+      # mat_texid (nmat, mjNTEXROLE): texture= fills the RGB role, each <layer texture= role=> its role
+      texid = [-1] * len(_TEX_ROLES)
+      for role, tex in [("rgb", ma.get("texture"))] + [(la.get("role", "rgb"), la.get("texture")) for la in me.findall("layer")]:
+        if tex is not None:
+          if role not in _TEX_ROLES:
+            raise ValueError(f"material layer role must be one of {list(_TEX_ROLES)}, got {role!r}")
+          texid[_TEX_ROLES.index(role)] = tex_names.index(tex) if tex in tex_names else len(tex_names)
+      mat_light.append((float(ma.get("specular", 0.5)), float(ma.get("shininess", 0.5)), float(ma.get("emission", 0.0)), *texid))
 
   def attrs(elem, childclass):
     cls = elem.get("class", childclass)
@@ -894,11 +940,13 @@ def compile_xml(root):
                           type=_GEOM_TYPES[a.get("type", "sphere")], size=ssize))
       elif tag == "camera":
         a = attrs(child, childclass)
-        cams.append(dict(name=a.get("name", f"cam{len(cams)}"), bodyid=bid, pos=_vec(a.get("pos"), default=[0, 0, 0]), quat=_frame_quat(a, compiler), mode=C.CAMLIGHT_MODES[a.get("mode", "fixed")], target=a.get("target")))
+        cams.append(dict(name=a.get("name", f"cam{len(cams)}"), bodyid=bid, pos=_vec(a.get("pos"), default=[0, 0, 0]), quat=_frame_quat(a, compiler), mode=C.CAMLIGHT_MODES[a.get("mode", "fixed")], target=a.get("target"),
+                         **_camera_optics(a)))
       elif tag == "light":
         a = attrs(child, childclass)
         d = _vec(a.get("dir"), default=[0, 0, -1])
-        lights.append(dict(name=a.get("name", f"light{len(lights)}"), bodyid=bid, pos=_vec(a.get("pos"), default=[0, 0, 0]), dir=d / np.linalg.norm(d), mode=C.CAMLIGHT_MODES[a.get("mode", "fixed")], target=a.get("target")))
+        lights.append(dict(name=a.get("name", f"light{len(lights)}"), bodyid=bid, pos=_vec(a.get("pos"), default=[0, 0, 0]), dir=d / np.linalg.norm(d), mode=C.CAMLIGHT_MODES[a.get("mode", "fixed")], target=a.get("target"),
+                           **_light_optics(a)))
       elif tag == "body":
         pass
       elif tag in ("flexcomp", "composite", "plugin"):
@@ -1096,6 +1144,9 @@ def compile_xml(root):
   m.geom_fluid = np.array([g["fluid"] for g in geoms]).reshape(ngeom, 12)
   m.nmat = len(mat_names)
   m.mat_rgba = np.array(mat_rgba).reshape(m.nmat, 4)
+  ml = np.array(mat_light, dtype=np.float64).reshape(m.nmat, 3 + len(_TEX_ROLES))
+  m.mat_specular, m.mat_shininess, m.mat_emission = ml[:, 0].copy(), ml[:, 1].copy(), ml[:, 2].copy()
+  m.mat_texid = ml[:, 3:].astype(np.int32)
   m.names.material = list(mat_names)
   m.geom_size = np.array([g["size"] for g in geoms]).reshape(ngeom, 3)
   m.geom_pos = np.array([g["pos"] for g in geoms]).reshape(ngeom, 3)
@@ -1178,6 +1229,17 @@ def compile_xml(root):
   m.light_targetbodyid = np.array([body_id(l["target"]) for l in lights], dtype=np.int32)
   m.light_pos = np.array([l["pos"] for l in lights]).reshape(m.nlight, 3)
   m.light_dir = np.array([l["dir"] for l in lights]).reshape(m.nlight, 3)
+  # the renderer's camera and light fields (MuJoCo's names and defaults)
+  for n, shape, dt in _CAMERA_FIELDS:
+    setattr(m, "cam_" + n, np.array([c[n] for c in cams], dtype=dt).reshape((m.ncam,) + shape))
+  for n, shape, dt in _LIGHT_FIELDS:
+    setattr(m, "light_" + n, np.array([l[n] for l in lights], dtype=dt).reshape((m.nlight,) + shape))
+  hl = dict(_HEADLIGHT_DEFAULTS)
+  vis_e = root.find("visual")
+  hl_e = vis_e.find("headlight") if vis_e is not None else None
+  if hl_e is not None:
+    hl.update({k: (int(hl_e.get(k)) if k == "active" else _vec(hl_e.get(k), 3)) for k in hl if k in hl_e.attrib})
+  m.vis = SimpleNamespace(headlight=SimpleNamespace(**hl))
 
   # ---- tendons: fixed tendons (linear combinations of scalar joint positions); spatial tendons are not compiled
   tens = []
@@ -1899,6 +1961,9 @@ def save_npz(m, path: str):
     if k in ("opt", "stat", "names"):
       for kk, vv in vars(v).items():
         out[f"{k}.{kk}"] = np.asarray(vv)
+    elif k == "vis":
+      for kk, vv in vars(v.headlight).items():
+        out[f"vis.headlight.{kk}"] = np.asarray(vv)
     else:
       out[k] = np.asarray(v)
   np.savez_compressed(path, **out)
@@ -1910,6 +1975,12 @@ def load_npz(path: str):
   for k in z.files:
     v = z[k]
     tgt, name = m, k
+    if k.startswith("vis.headlight."):
+      if not hasattr(m, "vis"):
+        m.vis = SimpleNamespace(headlight=SimpleNamespace())
+      tgt, name = m.vis.headlight, k[len("vis.headlight."):]
+      setattr(tgt, name, v.item() if v.ndim == 0 else v)
+      continue
     if "." in k:
       grp, name = k.split(".", 1)
       tgt = getattr(m, grp)

@@ -228,3 +228,16 @@ class Constraint(_Struct):
 
 class Data(_Struct):
   pass
+
+
+class RenderContext(_Struct):
+  """Render context of `create_render_context` (reference types.py RenderContext): the active cameras, their output buffers and
+  the enabled geoms.
+
+  nrender: active cameras; cam_id_map (nrender) their Model camera ids; cam_res (nrender, 2) width, height; pix_adr (nrender) first
+  pixel of each camera in `ray`; total_rays: pixels of all active cameras; ray (total_rays, 3) camera-frame ray directions (with
+  use_precomputed_rays); render_rgb / render_depth / render_seg (nrender) host bools; rgb_adr / depth_adr / seg_adr (nrender) first
+  pixel of each camera in rgb_data / depth_data / seg_data, -1 when the camera does not produce that output; rgb_data (nworld, nrgb)
+  uint32 packed 0xAARRGGBB; depth_data (nworld, ndepth) float32; seg_data (nworld, nseg, 2) int32 (geom id, mjOBJ_GEOM), (-1, -1) on a
+  miss; bvh_ngeom: enabled geoms; enabled_geom_ids (bvh_ngeom); lower / upper (nworld, bvh_ngeom, 3) world-space geom bounds written by
+  `refit_bvh`; mesh_bounds_size (nmesh, 3) half-extent of each mesh's vertex box; the remaining fields are the creation options."""

@@ -354,6 +354,45 @@ int mjb_rays(const mjbModel* m, mjbData* d, const float* pnt, const float* vec, 
   MJB_LAUNCH(launch_ray(m->dev, d->dev, pnt, vec, nray, pnt_nbatch, geomgroup, flg_static, bodyexclude, dist, geomid, normal, s));
   return 0;
 }
+static int check_render(const mjbModel* m, const mjbData* d, const mjbRender* rc, const char* what) {
+  if (!rc) return fail(std::string(what) + ": null render context");
+  if (rc->ngeom < 0 || rc->ncam < 0 || rc->npixel < 0) return fail(std::string(what) + ": negative size in the render context");
+  if (rc->ngeom > 0 && (!rc->geom_id || !rc->lower || !rc->upper)) return fail(std::string(what) + ": null geom table");
+  if (smem_render(rc->ngeom) > kMaxSmem)
+    return fail(std::string(what) + ": " + std::to_string(rc->ngeom) + " enabled geoms exceed one block's shared memory (at most " +
+                std::to_string(kMaxSmem / smem_render(1)) + ")");
+  if (rc->npixel > kRenderMaxPixels) return fail(std::string(what) + ": " + std::to_string(rc->npixel) + " pixels exceed " + std::to_string(kRenderMaxPixels));
+  if (rc->nlight != m->dev.nlight) return fail(std::string(what) + ": the render context has " + std::to_string(rc->nlight) + " lights, the model " + std::to_string(m->dev.nlight));
+  if (rc->nb_cam_fovy < 1 || rc->nb_cam_intrinsic < 1 || rc->nb_light_attenuation < 1 || rc->nb_light_cutoff < 1 || rc->nb_light_exponent < 1 ||
+      rc->nb_light_ambient < 1 || rc->nb_light_diffuse < 1 || rc->nb_light_specular < 1 || rc->nb_mat_specular < 1 || rc->nb_mat_shininess < 1 ||
+      rc->nb_mat_emission < 1)
+    return fail(std::string(what) + ": per-world field counts must be >= 1");
+  (void)d;
+  return 0;
+}
+int mjb_refit_bvh(const mjbModel* m, mjbData* d, const mjbRender* rc, void* stream) {
+  MJB_ENTER();
+  if (check_render(m, d, rc, "mjb_refit_bvh")) return -1;
+  MJB_LAUNCH(launch_refit_bvh(m->dev, d->dev, *rc, s));
+  return 0;
+}
+int mjb_render(const mjbModel* m, mjbData* d, const mjbRender* rc, void* stream) {
+  MJB_ENTER();
+  if (check_render(m, d, rc, "mjb_render")) return -1;
+  if (rc->npixel > 0 && (!rc->cam_id || !rc->cam_res || !rc->pix_adr || !rc->rgb_adr || !rc->depth_adr || !rc->seg_adr))
+    return fail("mjb_render: null camera table");
+  MJB_LAUNCH(launch_render(m->dev, d->dev, *rc, m->dev.nmesh > 0, s));
+  return 0;
+}
+int mjb_render_rays(const mjbRender* rc, float* ray, void* stream) {
+  g_launches = 0;
+  if (!rc || !ray) return fail("mjb_render_rays: null argument");
+  if (rc->npixel < 0 || rc->npixel > kRenderMaxPixels) return fail("mjb_render_rays: pixel count out of range: " + std::to_string(rc->npixel));
+  if (rc->npixel > 0 && (!rc->cam_id || !rc->cam_res || !rc->pix_adr || !rc->cam_projection || !rc->cam_fovy || !rc->cam_sensorsize || !rc->cam_intrinsic))
+    return fail("mjb_render_rays: null camera table");
+  MJB_LAUNCH(launch_render_rays(*rc, ray, (cudaStream_t)stream));
+  return 0;
+}
 // The k_energy parts of the position-stage sensors (sensor.py:845-849): the terms the energy sensors read, and the sensors themselves
 static int energy_sensor_parts(const mjbModel* m) {
   if (m->en.nsensor_energy == 0 || (m->dev.disableflags & DSBL_SENSOR)) return 0;

@@ -263,6 +263,13 @@ cudaError_t launch_rk_stage(const ModelDev& m, const DataDev& d, float* rk, int 
 // rays (nworld x nray, world-major) against every geom of every world; geomgroup: 6 ints, all -1 = no group filter (k_ray.cu)
 cudaError_t launch_ray(const ModelDev& m, const DataDev& d, const float* pnt, const float* vec, int nray, int pnt_nbatch, const int* geomgroup, int flg_static,
                        const int* bodyexclude, float* dist, int* geomid, float* normal, cudaStream_t s);
+// the batch renderer (k_render.cu): bounds of rc's enabled geoms in every world; one image per (world, active camera) of rc
+struct mjbRender;
+cudaError_t launch_refit_bvh(const ModelDev& m, const DataDev& d, const mjbRender& rc, cudaStream_t s);
+cudaError_t launch_render(const ModelDev& m, const DataDev& d, const mjbRender& rc, bool has_mesh, cudaStream_t s);
+cudaError_t launch_render_rays(const mjbRender& rc, float* ray, cudaStream_t s);  // the camera-frame ray table of rc's pixels
+size_t smem_render(int ngeom);
+constexpr int kRenderMaxPixels = 65535 * 128;  // pixels of all active cameras (tiles of 128 along the grid's y dimension)
 cudaError_t launch_ctrl_noise(const ModelDev& m, const DataDev& d, const float* ctrl_center, int step, float std, float rate, cudaStream_t s);
 size_t smem_position(const ModelDev& m, const DataDev& d);
 size_t smem_collision(const ModelDev& m, const DataDev& d);

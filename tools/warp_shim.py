@@ -111,6 +111,9 @@ class Mat:
 
   def __getitem__(self, idx):
     if isinstance(idx, tuple):
+      if isinstance(idx[0], slice):  # m[:, j]: a copy of column j
+        col = [r[idx[1]] for r in self.m[idx[0]]]
+        return _vec_cls(len(col))(col)
       return self.m[idx[0]][idx[1]]
     return _vec_cls(len(self.m[idx]))(list(self.m[idx]))  # a COPY of the row
 
@@ -249,6 +252,7 @@ def _build_warp():
   wp.normalize = normalize
   wp.cw_mul = lambda a, b: a._new([p * q for p, q in zip(a.v, b.v)])
   wp.sqrt, wp.sin, wp.cos, wp.atan2, wp.acos, wp.exp, wp.log, wp.pow = _m.sqrt, _m.sin, _m.cos, _m.atan2, _m.acos, _m.exp, _m.log, _m.pow
+  wp.tan = _m.tan  # render_util.py compute_ray
   wp.sign = lambda x: x._new([-1.0 if a < 0 else 1.0 for a in x.v]) if isinstance(x, Vec) else (-1.0 if x < 0 else 1.0)  # warp: sign(0) = +1
   wp.clamp = lambda x, lo, hi: min(max(x, lo), hi)
   wp.transpose = lambda a: _mat_cls(len(a.m[0]), len(a.m))._from_rows([list(c) for c in zip(*a.m)])
@@ -903,11 +907,129 @@ class _WarpSemantics(ast.NodeTransformer):
       return ast.copy_location(ast.Assign(targets=[node.target], value=ast.Call(func=ast.Name(id=fn, ctx=ast.Load()), args=[load, node.value], keywords=[])), node)
     return node
 
+  def visit_Call(self, node):
+    # warp's `bvh_query_next(query, index, max_dist)` writes `index` through a reference: rebound here from the query object
+    self.generic_visit(node)
+    f = node.func
+    if self.depth and isinstance(f, ast.Attribute) and f.attr == "bvh_query_next" and len(node.args) == 3 and isinstance(node.args[1], ast.Name):
+      q, idx, dist = node.args
+      nxt = ast.Call(func=f, args=[q, dist], keywords=[])
+      bind = ast.Compare(left=ast.NamedExpr(target=ast.Name(id=idx.id, ctx=ast.Store()), value=ast.Attribute(value=q, attr="index", ctx=ast.Load())),
+                         ops=[ast.IsNot()], comparators=[ast.Constant(value=None)])
+      return ast.copy_location(ast.BoolOp(op=ast.And(), values=[nxt, bind]), node)
+    return node
+
   def visit_Assign(self, node):
     self.generic_visit(node)
+    # warp's `hit = mesh_query_ray(id, p, v, max_t, t, u, v, sign, n, f)` writes its last six arguments through references
+    v = node.value
+    if (self.depth and isinstance(v, ast.Call) and isinstance(v.func, ast.Attribute) and v.func.attr == "mesh_query_ray" and len(v.args) == 10
+        and len(node.targets) == 1):
+      outs = [ast.Name(id=a.id, ctx=ast.Store()) for a in v.args[4:]]
+      node.targets = [ast.Tuple(elts=[node.targets[0]] + outs, ctx=ast.Store())]
+      v.args = v.args[:4]
+      return node
     if self.depth and isinstance(node.value, (ast.Name, ast.Attribute)):
       node.value = ast.copy_location(ast.Call(func=ast.Name(id="__wp_copy__", ctx=ast.Load()), args=[node.value], keywords=[]), node.value)
     return node
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# brute-force stand-ins for warp's BVH and mesh queries (the renderer: bvh.py, render.py, ray.py ray_mesh_with_bvh).  A BVH only
+# prunes candidates, so visiting every leaf whose bounds the ray enters gives the same closest hit (exact ties aside).
+_OBJECTS = {}
+
+
+def _register(obj):
+  obj.id = len(_OBJECTS) + 1
+  _OBJECTS[obj.id] = obj
+  return obj
+
+
+def _slab(lo, hi, p, v, max_t):
+  """the ray p + t v enters the box [lo, hi] at some t < max_t with the box not wholly behind its origin"""
+  tmin, tmax = -_m.inf, _m.inf
+  for k in range(3):
+    if v[k] != 0.0:
+      a, b = (lo[k] - p[k]) / v[k], (hi[k] - p[k]) / v[k]
+      tmin, tmax = max(tmin, min(a, b)), min(tmax, max(a, b))
+    elif p[k] < lo[k] or p[k] > hi[k]:
+      return False
+  return tmax >= max(tmin, 0.0) and tmin < max_t
+
+
+class _Bvh:
+  def __init__(self, lower, upper, groups=None, constructor=None, **kw):
+    self.lower, self.upper, self.groups = lower, upper, groups  # read live: refit() has nothing to do
+    _register(self)
+
+  def refit(self):
+    pass
+
+
+class _BvhQuery:
+  def __init__(self, bvh, p, v, root):
+    lo, hi = bvh.lower.numpy().reshape(-1, 3), bvh.upper.numpy().reshape(-1, 3)
+    grp = bvh.groups.numpy().reshape(-1) if bvh.groups is not None else _np.zeros(len(lo), dtype=int)
+    self.leaves = [(i, lo[i], hi[i]) for i in range(len(lo)) if int(grp[i]) == int(root)]
+    self.p, self.v, self.k, self.index = [float(x) for x in p], [float(x) for x in v], 0, -1
+
+  def next(self, max_t):
+    while self.k < len(self.leaves):
+      i, lo, hi = self.leaves[self.k]
+      self.k += 1
+      if _slab(lo, hi, self.p, self.v, max_t):
+        self.index = i
+        return True
+    return False
+
+
+class _Mesh:
+  def __init__(self, points=None, indices=None, **kw):
+    self.points = _np.asarray(points.numpy(), dtype=_np.float64).reshape(-1, 3)
+    self.tris = _np.asarray(indices.numpy(), dtype=_np.int64).reshape(-1, 3)
+    _register(self)
+
+
+def _mesh_query_ray(mesh_id, p, v, max_t):
+    """warp's mesh_query_ray: the closest triangle hit with 0 <= t < max_t, either side; (hit, t, u, v, sign, normal, face), with the
+    hit point u p0 + v p1 + (1 - u - v) p2 and the unit face normal cross(p1 - p0, p2 - p0)"""
+    mesh = _OBJECTS[int(mesh_id)]
+    o, d = _np.array([float(x) for x in p]), _np.array([float(x) for x in v])
+    best = None
+    for f, (i0, i1, i2) in enumerate(mesh.tris):
+      a, b, c = mesh.points[i0], mesh.points[i1], mesh.points[i2]
+      e1, e2 = b - a, c - a
+      h = _np.cross(d, e2)
+      det = e1 @ h
+      if det == 0.0:
+        continue
+      s = o - a
+      bu = (s @ h) / det
+      q = _np.cross(s, e1)
+      bv = (d @ q) / det
+      t = (e2 @ q) / det
+      if bu < 0.0 or bv < 0.0 or bu + bv > 1.0 or t < 0.0 or t >= max_t:
+        continue
+      if best is None or t < best[0]:
+        best = (t, 1.0 - bu - bv, bu, f)
+    vec3 = _vec_cls(3)
+    if best is None:
+      return False, 0.0, 0.0, 0.0, 0.0, vec3(0.0, 0.0, 0.0), -1
+    t, u, w, f = best
+    i0, i1, i2 = mesh.tris[f]
+    n = _np.cross(mesh.points[i1] - mesh.points[i0], mesh.points[i2] - mesh.points[i0])
+    n = n / _np.linalg.norm(n)
+    return True, t, u, w, (1.0 if n @ d < 0.0 else -1.0), vec3(*n), f
+
+
+def _install_render_stand_ins(wp):
+  wp.Bvh, wp.Mesh = _Bvh, _Mesh
+  wp.bvh_get_group_root = lambda bvh_id, group: int(group)
+  wp.bvh_query_ray = lambda bvh_id, p, v, root: _BvhQuery(_OBJECTS[int(bvh_id)], p, v, root)
+  wp.bvh_query_next = lambda query, max_t: query.next(max_t)
+  wp.mesh_query_ray = _mesh_query_ray
+  wp.mesh_query_ray_anyhit = lambda mesh_id, p, v, max_t: _mesh_query_ray(mesh_id, p, v, max_t)[0]
 
 
 def install(root="/root/reference/mujoco_warp/_src"):
@@ -917,6 +1039,7 @@ def install(root="/root/reference/mujoco_warp/_src"):
   import importlib.machinery
 
   wp = _build_warp()
+  _install_render_stand_ins(wp)
   sys.modules["warp"] = wp
   sys.modules["warp.types"] = wp.types
   pkg = _t.ModuleType("mujoco_warp")
