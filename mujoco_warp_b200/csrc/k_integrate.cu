@@ -215,10 +215,12 @@ k_next_act(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev 
 // rk: per world [qpos_t0 (nq) | qvel_t0 (nv) | qvel_rk (nv) | qacc_rk (nv) | act_t0 (na) | act_dot_rk (na)].  One warp per world.
 // Stateful actuators (forward.py:445-463, 514-519, 553-555): stage activations are next_act(act_t0, act_dot, A) without the range
 // clamp, the final ones next_act(act_t0, sum B act_dot, 1) with it.
+template <bool BAT>
 __global__ void __launch_bounds__(32)
-k_rk_stage(const __grid_constant__ ModelDev m, const __grid_constant__ DataDev d, float* __restrict__ rk, int stage) {
+k_rk_stage(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d, float* __restrict__ rk, int stage) {
   const int lane = threadIdx.x, w = blockIdx.x;
   if (w >= d.nworld) return;
+  MJB_WORLD_MODEL(w)
   const int nq = m.nq, nv = m.nv;
   const size_t wb = (size_t)w;
   const int na = m.na;
@@ -295,5 +297,5 @@ cudaError_t launch_ctrl_noise(const ModelDev& m, const DataDev& d, const float* 
 }
 
 cudaError_t launch_rk_stage(const ModelDev& m, const DataDev& d, float* rk, int stage, cudaStream_t s) {
-  return launch(k_rk_stage, d.nworld, 32, 0, s, m, d, rk, stage);
+  return launch(m.batched ? k_rk_stage<true> : k_rk_stage<false>, d.nworld, 32, 0, s, m, d, rk, stage);
 }

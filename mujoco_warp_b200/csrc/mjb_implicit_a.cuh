@@ -31,8 +31,9 @@ __device__ __forceinline__ void tree_implicit_a(const ModelDev& m, const DataDev
   if (implicitfast && m.nu > 0 && !(m.disableflags & DSBL_ACTUATION)) {
 #pragma unroll 1
     for (int a = 0; a < m.nu; a++) {  // actuators one after the other: fixed accumulation order, no atomics
-      const int adr = m.moment_rowadr0[a], nnz = m.moment_rownnz0[a], d0 = m.moment_colind0[adr];
-      if (d0 < start || d0 >= start + n) continue;
+      const int adr = m.moment_rowadr0[a], nnz = m.moment_rownnz0[a];
+      // moment_colind0 rows are ascending: skip an actuator with no dof in [start, start + n); one that spans trees stays
+      if (nnz == 0 || m.moment_colind0[adr + nnz - 1] < start || m.moment_colind0[adr] >= start + n) continue;
       const float gain = m.actuator_gaintype[a] == GAIN_AFFINE ? m.actuator_gainprm[10 * a + 2] : 0.f;
       const float bias = m.actuator_biastype[a] == BIAS_AFFINE ? m.actuator_biasprm[10 * a + 2] : 0.f;
       if (bias == 0.f && gain == 0.f) continue;
@@ -51,9 +52,10 @@ __device__ __forceinline__ void tree_implicit_a(const ModelDev& m, const DataDev
       for (int p = lane; p < nnz * nnz; p += 32) {
         const int i = p / nnz, j = p - i * nnz;
         const int di = m.moment_colind0[adr + i], dj = m.moment_colind0[adr + j];
-        // entries of the M sparsity pattern only (derivative.py:178-218: M_elemid < 0 is skipped): dj is di or an ancestor dof
-        // of it -- a tendon transmission may couple dofs of sibling bodies, which M does not
-        if (j <= i && m.body_isdofancestor[m.dof_bodyid[di] * nv + dj]) {
+        // entries of this tree's block of the M sparsity pattern only (derivative.py:178-218: M_elemid < 0 is skipped): di in the
+        // block, dj di or an ancestor dof of it -- a tendon transmission may couple dofs of sibling bodies or of other trees, which
+        // M does not
+        if (j <= i && di >= start && di < start + n && m.body_isdofancestor[m.dof_bodyid[di] * nv + dj]) {
           const float mi = d.actuator_moment[wb * m.nJmom + adr + i], mj = d.actuator_moment[wb * m.nJmom + adr + j];
           A[(di - start) * ld + (dj - start)] -= dt * mi * mj * vel;
         }
