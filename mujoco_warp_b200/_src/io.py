@@ -424,6 +424,39 @@ def history_fields(mjm) -> dict:
   )
 
 
+def _contact_sensor_intprm(mjm) -> np.ndarray:
+  """sensor_intprm (nsensor, 3) of a model, after checking every <contact> sensor's entries: known data bits and reduce, num >= 1, dim
+  equal to num times the slot size, and objects of the kinds and ranges the compiler emits.  ValueError naming the sensor otherwise."""
+  ns = int(getattr(mjm, "nsensor", 0))
+  stype = np.asarray(mjm.sensor_type).reshape(ns) if ns else np.zeros(0, dtype=int)
+  intprm = np.asarray(getattr(mjm, "sensor_intprm", np.zeros((ns, 3))), dtype=np.int64).reshape(ns, -1)[:, :3] if ns else np.zeros((0, 3))
+  names = list(getattr(getattr(mjm, "names", None), "sensor", None) or [f"sensor{i}" for i in range(ns)])
+  counts = {C.OBJ_SITE: int(getattr(mjm, "nsite", 0)), C.OBJ_GEOM: int(mjm.ngeom), C.OBJ_BODY: int(mjm.nbody), C.OBJ_XBODY: int(mjm.nbody)}
+  for s in np.nonzero(stype == C.SENS_CONTACT)[0]:
+    what = f"contact sensor '{names[s]}'"
+    dataspec, reduce, num = (int(x) for x in intprm[s])
+    if dataspec < 1 or dataspec >= 1 << len(mjcf.CONTACT_DATA):
+      raise ValueError(f"{what}: unknown data bits {dataspec:#x} (found force torque dist pos normal tangent are bits 0-6)")
+    if not 0 <= reduce < len(mjcf.CONTACT_REDUCE):
+      raise ValueError(f"{what}: unknown reduce {reduce} (expected 0 none, 1 mindist, 2 maxforce or 3 netforce)")
+    if num < 1:
+      raise ValueError(f"{what}: num must be >= 1, got {num}")
+    if int(mjm.sensor_dim[s]) != num * mjcf.contact_slot_size(dataspec):
+      raise ValueError(f"{what}: dim {int(mjm.sensor_dim[s])} is not num ({num}) x the slot size ({mjcf.contact_slot_size(dataspec)}) of its data")
+    for side, kinds, typ, oid in ((1, (C.OBJ_SITE, C.OBJ_GEOM, C.OBJ_BODY, C.OBJ_XBODY), int(mjm.sensor_objtype[s]), int(mjm.sensor_objid[s])),
+                                  (2, (C.OBJ_GEOM, C.OBJ_BODY, C.OBJ_XBODY), int(getattr(mjm, "sensor_reftype", np.zeros(ns))[s]), int(getattr(mjm, "sensor_refid", -np.ones(ns))[s]))):
+      if typ == C.OBJ_UNKNOWN:
+        continue
+      if typ not in kinds:
+        raise ValueError(f"{what}: side {side} has object type {typ}; expected none or one of {kinds}")
+      if not 0 <= oid < counts[typ]:
+        raise ValueError(f"{what}: side {side} names an unknown object (id {oid})")
+  out = np.zeros((ns, 3), dtype=np.int32)
+  contact = stype == C.SENS_CONTACT
+  out[contact] = intprm[contact]
+  return out
+
+
 def _validate_history(mjm):
   """Refuses, by name, delays and intervals the history buffers would not honour: the reference silently reads the undelayed value
   when nsample is 0 (history.py:380), and negative sizes / times have no meaning."""
@@ -613,6 +646,12 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   stype = np.asarray(mjm.sensor_type) if nsensor else np.zeros(0, dtype=int)
   m.sensor_subtree_vel = bool(np.isin(stype, (C.SENS_SUBTREELINVEL, C.SENS_SUBTREEANGMOM)).any())  # reference io.py:896-897
   m.sensor_rne_postconstraint = bool(np.isin(stype, (C.SENS_ACCELEROMETER, C.SENS_FORCE, C.SENS_TORQUE, C.SENS_FRAMELINACC, C.SENS_FRAMEANGACC)).any())  # :900
+  # <contact> sensors (reference io.py:409-413, :441, :898): their ids, [dataspec, reduce, num] per sensor, and the match capacity
+  sensor_intprm = _contact_sensor_intprm(mjm)
+  m.sensor_intprm = dev_i(sensor_intprm)
+  m.sensor_contact_adr = dev_i(np.nonzero(stype == C.SENS_CONTACT)[0])
+  m.nsensorcontact = int(m.sensor_contact_adr.numel())
+  m.opt.contact_sensor_maxmatch = mjcf.contact_sensor_maxmatch(mjm)
   sc = _sensor_collision_tables(mjm, t)
   m.nsensorcollision, m.sensor_collision_epa_iterations, m.nsensorcollision_ccd = (sc.pop(k) for k in ("nsensorcollision", "sensor_collision_epa_iterations", "nsensorcollision_ccd"))
   for n, x in sc.items():
@@ -708,7 +747,7 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   for k, v in (("nsensorcollision", m.nsensorcollision), ("nsensorcollision_sensor", len(m.sensor_collision_id)), ("sensor_collision_epa_iterations", m.sensor_collision_epa_iterations),
                ("nsensorcollision_ccd", m.nsensorcollision_ccd), ("nsensor_energy", len(t["sensor_energy_adr"])),
                ("sensor_e_potential", m.sensor_e_potential), ("sensor_e_kinetic", m.sensor_e_kinetic),
-               ("nhistory", m.nhistory), ("nactuator_history", int((hf["actuator_history"][:, 0] > 0).sum())), ("nsensor_history", len(m.sensor_history_id))):
+               ("nsensorcontact", m.nsensorcontact), ("contact_sensor_maxmatch", m.opt.contact_sensor_maxmatch), ("nhistory", m.nhistory), ("nactuator_history", int((hf["actuator_history"][:, 0] > 0).sum())), ("nsensor_history", len(m.sensor_history_id))):
     _lib.check(L.mjb_model_set_int(h, k.encode(), int(v)))
   g = np.asarray(o.gravity, dtype=np.float64)
   floats = dict(timestep=o.timestep, tolerance=tol, ls_tolerance=o.ls_tolerance, impratio_invsqrt=1.0 / np.sqrt(o.impratio),
@@ -735,7 +774,7 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
                                          "geom_fluid", "body_fluid", "body_geomadr", "body_geomnum", "sensor_collision_start_adr", "sensor_collision_pair",
                                          "sensor_collision_id", "sensor_collision_adr", "sensor_collision_flip", "actuator_acc0", "actuator_lengthrange", "jnt_limited", "sensor_energy_adr",
                                          "actuator_history", "actuator_historyadr", "actuator_delay", "sensor_history", "sensor_historyadr", "sensor_delay",
-                                         "sensor_interval", "sensor_history_id"]
+                                         "sensor_interval", "sensor_history_id", "sensor_contact_adr", "sensor_intprm"]
                                         + [n for n, _ in _TENDON_FLOATS]):
     dev_names.setdefault(n, getattr(m, n))
   for n, x in dev_names.items():
@@ -752,7 +791,8 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
 
 _OPT_FLOATS = {"timestep": "timestep", "tolerance": "tolerance", "ls_tolerance": "ls_tolerance", "impratio_invsqrt": "impratio_invsqrt", "ccd_tolerance": "ccd_tolerance",
                "density": "density", "viscosity": "viscosity"}
-_OPT_INTS = ("integrator", "cone", "solver", "iterations", "ls_iterations", "disableflags", "enableflags", "broadphase", "broadphase_filter", "ccd_iterations")
+_OPT_INTS = ("integrator", "cone", "solver", "iterations", "ls_iterations", "disableflags", "enableflags", "broadphase", "broadphase_filter", "ccd_iterations",
+             "contact_sensor_maxmatch")
 
 
 def _check_like(name, new, old):
@@ -801,6 +841,8 @@ def _install_model_rebind(m: types.Model, L, arrays, ints):
     if name in _OPT_INTS:
       if name == "integrator" and int(value) not in (C.INT_EULER, C.INT_IMPLICIT, C.INT_IMPLICITFAST, C.INT_RK4):
         raise NotImplementedError(f"integrator {value} not implemented")
+      if name == "contact_sensor_maxmatch" and int(value) < 1:
+        raise ValueError(f"opt.contact_sensor_maxmatch must be >= 1, got {int(value)}")
       if name in ("integrator", "cone", "solver") and int(value) != int(m.opt.__dict__[name]):
         raise NotImplementedError(f"opt.{name} selects kernel instantiations and scratch sizes fixed at put_model / make_data; rebuild the Model to change it")
       _lib.check(L.mjb_model_set_int(h, name.encode(), int(value)))

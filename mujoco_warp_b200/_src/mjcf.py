@@ -290,6 +290,55 @@ def _geom_aabb(gtype, size):
 _ACT_TAGS = ("general", "motor", "position", "velocity", "intvelocity", "damper", "cylinder", "muscle", "adhesion")
 # the <muscle> shortcut's scalar parameters after range, in gainprm / biasprm order, with MuJoCo's defaults
 _MUSCLE_DEFAULTS = (("force", -1.0), ("scale", 200.0), ("lmin", 0.5), ("lmax", 1.6), ("vmax", 1.5), ("fpmax", 1.3), ("fvmax", 1.2))
+# <contact> sensor: data keywords in their canonical order (bit i of sensor_intprm[0]) with the floats each adds to a slot, and the
+# reductions (sensor_intprm[1]); reference sensor.py:1816-1851, :2448-2494
+CONTACT_DATA = (("found", 1), ("force", 3), ("torque", 3), ("dist", 1), ("pos", 3), ("normal", 3), ("tangent", 3))
+CONTACT_REDUCE = ("none", "mindist", "maxforce", "netforce")
+CONTACT_SENSOR_MAXMATCH = 64  # matches kept per contact sensor and world unless <numeric name="contact_sensor_maxmatch"> says otherwise
+
+
+def contact_slot_size(dataspec: int) -> int:
+  return sum(n for i, (_, n) in enumerate(CONTACT_DATA) if dataspec >> i & 1)
+
+
+def contact_intprm(data, reduce, num, what):
+  """(dataspec, reduce, num) of a <contact> sensor's data / reduce / num attributes; ValueError naming `what` for an unknown or
+  out-of-order data keyword, an unknown reduce value or num < 1."""
+  keys = [k for k, _ in CONTACT_DATA]
+  words = str(data).split()
+  if not words:
+    raise ValueError(f"{what}: data must list at least one of {' '.join(keys)}")
+  for w in words:
+    if w not in keys:
+      raise ValueError(f"{what}: unknown data keyword '{w}' (expected some of {' '.join(keys)}, in that order)")
+  idx = [keys.index(w) for w in words]
+  if any(b <= a for a, b in zip(idx, idx[1:])):
+    raise ValueError(f"{what}: data keywords '{data}' must appear once each, in the order {' '.join(keys)}")
+  if reduce not in CONTACT_REDUCE:
+    raise ValueError(f"{what}: unknown reduce '{reduce}' (expected one of {', '.join(CONTACT_REDUCE)})")
+  try:
+    n = int(num)
+  except ValueError:
+    raise ValueError(f"{what}: num must be an integer >= 1, got '{num}'") from None
+  if n < 1:
+    raise ValueError(f"{what}: num must be >= 1, got {n}")
+  return (sum(1 << i for i in idx), CONTACT_REDUCE.index(reduce), n)
+
+
+def contact_sensor_maxmatch(mjm) -> int:
+  """Option.contact_sensor_maxmatch of a compiled model: its <numeric name="contact_sensor_maxmatch"> (reference io.py:409-413), else 64"""
+  names = list(getattr(getattr(mjm, "names", None), "numeric", None) or [])
+  if "contact_sensor_maxmatch" not in names:
+    return CONTACT_SENSOR_MAXMATCH
+  i = names.index("contact_sensor_maxmatch")
+  if int(mjm.numeric_size[i]) < 1:
+    raise ValueError('numeric contact_sensor_maxmatch: needs one value (data="N")')
+  v = float(mjm.numeric_data[int(mjm.numeric_adr[i])])
+  if v != int(v) or v < 1:
+    raise ValueError(f"numeric contact_sensor_maxmatch: must be an integer >= 1, got {v:g}")
+  return int(v)
+
+
 # delay / history attributes of actuators and sensors; interp keywords as in the reference's history.py:88 (0 zoh, 1 linear, 2 cubic)
 _HISTORY_KEYS = ("nsample", "interp", "delay", "interval")
 _INTERP = {"zoh": 0, "linear": 1, "cubic": 2}
@@ -1583,10 +1632,14 @@ def compile_xml(root):
     "distance": (S.SENS_GEOMDIST, "pair", 1, 0, 1), "normal": (S.SENS_GEOMNORMAL, "pair", 3, 2, 1), "fromto": (S.SENS_GEOMFROMTO, "pair", 6, 0, 1),
     # potential and kinetic energy of the whole model (no object)
     "e_potential": (S.SENS_E_POTENTIAL, None, 1, 0, 1), "e_kinetic": (S.SENS_E_KINETIC, None, 1, 0, 1),
+    # contacts matched against up to two sides; dim is num x the slot size of its data keywords (below)
+    "contact": (S.SENS_CONTACT, "contact", 0, 0, 3),
   }
   objkind = {"tendon": (C.OBJ_TENDON, "tendon"), "joint": (C.OBJ_JOINT, "joint"), "actuator": (C.OBJ_ACTUATOR, "actuator"), "site": (C.OBJ_SITE, "site"), "body": (C.OBJ_BODY, "body")}
   objtypes = {"body": (C.OBJ_BODY, "body"), "xbody": (C.OBJ_XBODY, "body"), "geom": (C.OBJ_GEOM, "geom"), "site": (C.OBJ_SITE, "site"), "camera": (C.OBJ_CAMERA, "camera")}
   sens, unsupported = [], []
+  contact_sides = ((("site", C.OBJ_SITE), ("geom1", C.OBJ_GEOM), ("body1", C.OBJ_BODY), ("subtree1", C.OBJ_XBODY)),
+                   (("geom2", C.OBJ_GEOM), ("body2", C.OBJ_BODY), ("subtree2", C.OBJ_XBODY)))
   nsens = root.find("sensor")
   for e in (list(nsens) if nsens is not None else []):
     has_ref = "reftype" in e.attrib or "refname" in e.attrib
@@ -1609,6 +1662,25 @@ def compile_xml(root):
         otype_k, lst = objtypes[given[0]]
         sides.append((otype_k, getattr(m.names, lst).index(e.get(given[0] + k))))
       (otype, oid), (rtype, rid) = sides
+    elif kind == "contact":
+      sname = e.get("name", f"sensor{len(sens)}")
+      sides = []
+      for side in contact_sides:
+        given = [(a, t) for a, t in side if a in e.attrib]
+        if len(given) > 1:
+          raise ValueError(f"contact sensor '{sname}': give at most one of {' / '.join(a for a, _ in side)}, got {' and '.join(a for a, _ in given)}")
+        if not given:
+          sides.append((C.OBJ_UNKNOWN, -1))
+          continue
+        attr, t = given[0]
+        lst = {C.OBJ_SITE: "site", C.OBJ_GEOM: "geom"}.get(t, "body")
+        names = getattr(m.names, lst)
+        if e.get(attr) not in names:
+          raise ValueError(f"contact sensor '{sname}': unknown {lst} '{e.get(attr)}' in {attr}")
+        sides.append((t, names.index(e.get(attr))))
+      (otype, oid), (rtype, rid) = sides
+      intprm = contact_intprm(e.get("data", "found"), e.get("reduce", "none"), e.get("num", "1"), f"contact sensor '{sname}'")
+      dim = intprm[2] * contact_slot_size(intprm[0])
     elif kind == "obj":
       otype, lst = objtypes[e.get("objtype")]
       oid = getattr(m.names, lst).index(e.get("objname"))
@@ -1620,12 +1692,14 @@ def compile_xml(root):
     ha.update(e.attrib)
     hist, delay, interval = _history_attrs(ha, f"sensor '{sname}'", interval=True)
     sens.append(dict(name=sname, type=stype, objtype=otype, objid=oid, reftype=rtype, refid=rid, dim=dim, datatype=datatype, needstage=stage,
-                     cutoff=float(e.get("cutoff", 0.0)), noise=float(e.get("noise", 0.0)), history=hist, delay=delay, interval=interval))
+                     cutoff=float(e.get("cutoff", 0.0)), noise=float(e.get("noise", 0.0)), history=hist, delay=delay, interval=interval,
+                     intprm=intprm if kind == "contact" else (0, 0, 0)))
   m.nsensor = len(sens)
   m.sensor_unsupported = unsupported  # put_model refuses these (they would silently read zero otherwise)
   m.names.sensor = [x["name"] for x in sens]
   for key in ("type", "objtype", "objid", "reftype", "refid", "dim", "datatype", "needstage"):
     setattr(m, "sensor_" + key, np.array([x[key] for x in sens], dtype=np.int32).reshape(m.nsensor))
+  m.sensor_intprm = np.array([x["intprm"] for x in sens], dtype=np.int32).reshape(m.nsensor, 3)
   m.sensor_cutoff = np.array([x["cutoff"] for x in sens], dtype=np.float64).reshape(m.nsensor)
   m.sensor_noise = np.array([x["noise"] for x in sens], dtype=np.float64).reshape(m.nsensor)
   m.sensor_adr = (np.concatenate(([0], np.cumsum(m.sensor_dim)[:-1])) if m.nsensor else np.zeros(0)).astype(np.int32)
@@ -1634,6 +1708,19 @@ def compile_xml(root):
   m.sensor_delay = np.array([x["delay"] for x in sens], dtype=np.float64).reshape(m.nsensor)
   m.sensor_interval = np.array([x["interval"] for x in sens], dtype=np.float64).reshape(m.nsensor, 2)
   set_history_layout(m)
+
+  # ---- <custom><numeric>: MjModel's numeric_adr / numeric_size / numeric_data; the contact sensors read contact_sensor_maxmatch from it
+  nums = [n for c in root.findall("custom") for n in c.findall("numeric")]
+  vals = [np.array([float(x) for x in n.get("data", "").split()], dtype=np.float64) for n in nums]
+  for n, v in zip(nums, vals):
+    size = int(n.get("size", len(v)))
+    v.resize(max(size, len(v)), refcheck=False)
+  m.nnumeric = len(nums)
+  m.names.numeric = [n.get("name", "") for n in nums]
+  m.numeric_size = np.array([len(v) for v in vals], dtype=np.int32)
+  m.numeric_adr = (np.concatenate(([0], np.cumsum(m.numeric_size)[:-1])) if nums else np.zeros(0)).astype(np.int32)
+  m.numeric_data = np.concatenate(vals) if nums else np.zeros(0)
+  contact_sensor_maxmatch(m)
 
   # ---- keyframes
   keys = []

@@ -14,6 +14,7 @@ struct mjbModel {
   ModelDev dev;
   FluidDev fluid;  // qfrc_fluid stays null here: it is the Data's (fluid() below)
   SensorCollisionDev sc;
+  SensorContactDev scon;  // the <contact> sensors and Option.contact_sensor_maxmatch
   SetConstDev setc;  // actuator_acc0 and the meaninertia output, bound by name; qpos_save stays null here (the Data's)
   EnergyDev en;      // the energy sensors; energy stays null here (the Data's: energy() below)
   HistoryDev hist;   // the delay fields; history and ctrl_delayed stay null here (the Data's: history() below)
@@ -66,6 +67,7 @@ mjbModel* mjb_model_create(void) {
   memset(&m->dev, 0, sizeof(ModelDev));
   memset(&m->fluid, 0, sizeof(FluidDev));
   memset(&m->sc, 0, sizeof(SensorCollisionDev));
+  memset(&m->scon, 0, sizeof(SensorContactDev));
   memset(&m->setc, 0, sizeof(SetConstDev));
   memset(&m->en, 0, sizeof(EnergyDev));
   memset(&m->hist, 0, sizeof(HistoryDev));
@@ -84,6 +86,15 @@ int mjb_model_set_int(mjbModel* m, const char* name, int v) {
 #define X(n) if (!strcmp(name, #n)) { m->sc.n = v; return 0; }
   MJB_SENSCOL_INTS(X)
 #undef X
+  if (!strcmp(name, "contact_sensor_maxmatch")) {
+    SensorContactDev c = m->scon;
+    c.contact_sensor_maxmatch = v;
+    if (v < 1 || smem_sensor_contact(c) > kMaxSmem)
+      return fail("contact_sensor_maxmatch must be in [1, " + std::to_string(kMaxSmem / smem_sensor_contact(SensorContactDev{0, 1, nullptr, nullptr})) + "], got " + std::to_string(v));
+    m->scon.contact_sensor_maxmatch = v;
+    return 0;
+  }
+  if (!strcmp(name, "nsensorcontact")) { m->scon.nsensorcontact = v; return 0; }
 #define X(n) if (!strcmp(name, #n)) { m->en.n = v; return 0; }
   MJB_ENERGY_INTS(X)
 #undef X
@@ -112,6 +123,9 @@ int mjb_model_set_array_batched(mjbModel* m, const char* name, const void* p, in
 #undef X
 #define X(n) if (!strcmp(name, #n)) { if (nbatch != 1) return fail(std::string("shared by all worlds (not batched): ") + name); m->sc.n = (const int*)p; return 0; }
   MJB_SENSCOL_IARRS(X)
+#undef X
+#define X(n) if (!strcmp(name, #n)) { if (nbatch != 1) return fail(std::string("shared by all worlds (not batched): ") + name); m->scon.n = (const int*)p; return 0; }
+  MJB_SENSCON_IARRS(X)
 #undef X
 #define X(n) if (!strcmp(name, #n)) { if (nbatch != 1) return fail(std::string("shared by all worlds (not batched): ") + name); m->en.n = (const int*)p; return 0; }
   MJB_ENERGY_IARRS(X)
@@ -154,6 +168,10 @@ int mjb_model_finalize(mjbModel* m) {
 #define X(n) if (!m->sc.n) return fail(std::string("model array not set: ") + #n);
   MJB_SENSCOL_IARRS(X)
 #undef X
+#define X(n) if (!m->scon.n) return fail(std::string("model array not set: ") + #n);
+  MJB_SENSCON_IARRS(X)
+#undef X
+  if (m->scon.contact_sensor_maxmatch < 1) return fail("model int not set: contact_sensor_maxmatch");
 #define X(n) if (!m->en.n) return fail(std::string("model array not set: ") + #n);
   MJB_ENERGY_IARRS(X)
 #undef X
@@ -394,6 +412,15 @@ int mjb_render_rays(const mjbRender* rc, float* ray, void* stream) {
   return 0;
 }
 // The k_energy parts of the position-stage sensors (sensor.py:845-849): the terms the energy sensors read, and the sensors themselves
+// The sensors of `stages` (1 pos, 2 vel, 4 acc) for dd's world range: k_sensor (with the collision sensors for the position stage), then
+// for the acceleration stage the <contact> sensors (sensor.py:2605-2658), which read the solver's efc_force.  A model without contact
+// sensors launches what it launched before they existed.
+static cudaError_t sensors(const mjbModel* m, const DataDev& dd, int stages, cudaStream_t s) {
+  const cudaError_t e = launch_sensor(m->dev, dd, stages, s, m->sc);
+  if (e != cudaSuccess || m->dev.nsensor == 0 || !(stages & 4) || m->scon.nsensorcontact == 0 || (m->dev.disableflags & DSBL_SENSOR)) return e;
+  return launch_sensor_contact(m->dev, dd, m->scon, s);
+}
+
 static int energy_sensor_parts(const mjbModel* m) {
   if (m->en.nsensor_energy == 0 || (m->dev.disableflags & DSBL_SENSOR)) return 0;
   return ENERGY_SENSOR | (m->en.sensor_e_potential ? ENERGY_POT : 0) | (m->en.sensor_e_kinetic ? ENERGY_KIN : 0);
@@ -409,7 +436,7 @@ static int energy_forward_parts(const mjbModel* m) {
 
 int mjb_sensor_pos(const mjbModel* m, mjbData* d, void* stream) {
   MJB_ENTER();
-  MJB_LAUNCH(launch_sensor(m->dev, d->dev, 1, s, m->sc));
+  MJB_LAUNCH(sensors(m, d->dev, 1, s));
   MJB_LAUNCH(launch_energy(m->dev, d->dev, energy(m, d), energy_sensor_parts(m), s));
   MJB_LAUNCH(history_sensor(m, d, d->dev, 1, s));
   return 0;
@@ -418,13 +445,13 @@ int mjb_energy_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); M
 int mjb_energy_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_energy(m->dev, d->dev, energy(m, d), ENERGY_KIN, s)); return 0; }
 int mjb_sensor_vel(const mjbModel* m, mjbData* d, void* stream) {
   MJB_ENTER();
-  MJB_LAUNCH(launch_sensor(m->dev, d->dev, 2, s, m->sc));
+  MJB_LAUNCH(sensors(m, d->dev, 2, s));
   MJB_LAUNCH(history_sensor(m, d, d->dev, 2, s));
   return 0;
 }
 int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream) {
   MJB_ENTER();
-  MJB_LAUNCH(launch_sensor(m->dev, d->dev, 4, s, m->sc));
+  MJB_LAUNCH(sensors(m, d->dev, 4, s));
   MJB_LAUNCH(history_sensor(m, d, d->dev, 4, s));
   return 0;
 }
@@ -469,7 +496,7 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
   if (what & RUN_SOLVER) {
     MJB_LAUNCH(launch_solver(m->dev, dd, s));
     // sensors of all three stages in one launch after the solver (forward.py:1350-1365 interleaves them; their inputs are final by now)
-    if (m->dev.nsensor > 0) MJB_LAUNCH(launch_sensor(m->dev, dd, 7, s, m->sc));
+    if (m->dev.nsensor > 0) MJB_LAUNCH(sensors(m, dd, 7, s));
     // energy after the sensors (the reference's energy_pos / energy_vel, forward.py:1327-1356): its inputs are final since fwd_velocity
     MJB_LAUNCH(launch_energy(m->dev, dd, energy(m, d), energy_forward_parts(m), s));
     MJB_LAUNCH(history_sensor(m, d, dd, 7, s));  // after every kernel that writes sensordata
@@ -483,7 +510,7 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
     if (m->dev.nsensor > 0) {
       DataDev ds = dd;
       if (disc) ds.qacc = d->inv_qacc;
-      MJB_LAUNCH(launch_sensor(m->dev, ds, 7, s, m->sc));
+      MJB_LAUNCH(sensors(m, ds, 7, s));
     }
     MJB_LAUNCH(launch_energy(m->dev, dd, energy(m, d), energy_sensor_parts(m), s));  // inverse computes energy only for its sensors
     MJB_LAUNCH(history_sensor(m, d, dd, 7, s));

@@ -5,6 +5,7 @@
 // symmetric gather tables of io.py:1029-1050).  One warp per world, like every other stage.
 #include "mjb_launch.cuh"
 #include "mjb_math.cuh"
+#include "mjb_sensor_contact.cuh"
 #include "mjb_types.cuh"
 
 namespace {
@@ -125,7 +126,7 @@ k_mul_m(const __grid_constant__ ModelDev m, const __grid_constant__ DataDev d, f
 }
 
 // support.py:326-442 contact_force: 6D force / torque of the listed contacts, in the contact frame unless to_world is set
-// (pyramid decode :326-348; elliptic rows are the force components themselves).  No adhesion in this build.
+// (the decode is mjb_sensor_contact.cuh's contact_force_decode).  No adhesion in this build.
 __global__ void k_contact_force(const __grid_constant__ ModelDev m, const __grid_constant__ DataDev d, const int* __restrict__ contact_ids, int n, int to_world,
                                 float* __restrict__ out) {
   const int tid = blockIdx.x * blockDim.x + threadIdx.x;
@@ -134,23 +135,9 @@ __global__ void k_contact_force(const __grid_constant__ ModelDev m, const __grid
   if (cid >= d.nacon[0]) return;
   float f[6] = {0.f, 0.f, 0.f, 0.f, 0.f, 0.f};
   if (cid >= 0) {
-    const int w = d.contact_worldid[cid], dim = d.contact_dim[cid];
-    const int* adr = d.contact_efc_address + (size_t)cid * m.nmaxpyramid;
-    const float* force = d.efc_force + (size_t)w * d.njmax;
-    if (adr[0] >= 0) {
-      if (m.cone == CONE_PYRAMIDAL) {
-        if (dim == 1) f[0] = force[adr[0]];
-        else
-          for (int i = 0; i < dim - 1; i++) {
-            const int a = 2 * i + adr[0];
-            const float d1 = a < d.njmax ? force[a] : 0.f, d2 = a + 1 < d.njmax ? force[a + 1] : 0.f;
-            f[0] += d1 + d2;
-            f[i + 1] = (d1 - d2) * d.contact_friction[5 * (size_t)cid + i];
-          }
-      } else {
-        for (int i = 0; i < dim; i++) if (adr[i] < d.njmax) f[i] = force[adr[i]];
-      }
-    }
+    const int w = d.contact_worldid[cid];
+    contact_force_decode(m.cone, d.njmax, d.efc_force + (size_t)w * d.njmax, d.contact_efc_address + (size_t)cid * m.nmaxpyramid,
+                         d.contact_friction + 5 * (size_t)cid, d.contact_dim[cid], f);
     if (to_world) {  // row vector times the frame matrix, for the force and the torque part
       const float* R = d.contact_frame + 9 * (size_t)cid;
       float t[6];

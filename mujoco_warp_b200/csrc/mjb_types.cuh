@@ -147,6 +147,18 @@ struct SensorCollisionDev {
   const int* __restrict__ sensor_collision_flip;       // (like start_adr) the entry's geom1 is the narrowphase's second geom
 };
 
+// ---------------------------------------------------------------- contact sensors (k_sensor_contact.cu, mjb_sensor_contact.cuh)
+// The <contact> sensors' tables and Option.contact_sensor_maxmatch, passed as one extra argument to k_sensor_contact only, for the same
+// reason as FluidDev.
+#define MJB_SENSCON_INTS(X) X(nsensorcontact) X(contact_sensor_maxmatch)
+#define MJB_SENSCON_IARRS(X) X(sensor_contact_adr) X(sensor_intprm)
+struct SensorContactDev {
+  int nsensorcontact;                          // contact sensors
+  int contact_sensor_maxmatch;                 // matches kept per sensor and world (the rest are counted, and raise OVF_CONTACT_MATCH)
+  const int* __restrict__ sensor_contact_adr;  // (nsensorcontact) their sensor ids
+  const int* __restrict__ sensor_intprm;       // (nsensor, 3) dataspec, reduce, num of each contact sensor; zeros for the others
+};
+
 // ---------------------------------------------------------------- set_const (k_set_const.cu)
 // The fields of mjb_set_const that are neither in ModelDev nor in DataDev, passed as one extra argument to its kernels only, for the
 // same reason as FluidDev.  Writes to the other derived Model fields go through ModelDev's pointers and nb_* / bs_*.
@@ -220,7 +232,7 @@ enum {
   DSBL_ACTUATION = 1 << 11, DSBL_REFSAFE = 1 << 12, DSBL_SENSOR = 1 << 13, DSBL_EULERDAMP = 1 << 15, DSBL_NATIVECCD = 1 << 17
 };
 enum { ENBL_ENERGY = 1 << 1, ENBL_INVDISCRETE = 1 << 3 };
-enum { OVF_NEFC = 1 << 0, OVF_NJMAX_NNZ = 1 << 1, OVF_BROADPHASE = 1 << 2, OVF_NARROWPHASE = 1 << 3, OVF_EPA_HORIZON = 1 << 8, OVF_ITERATIONS = 1 << 9, OVF_LS_ITERATIONS = 1 << 10 };
+enum { OVF_NEFC = 1 << 0, OVF_NJMAX_NNZ = 1 << 1, OVF_BROADPHASE = 1 << 2, OVF_NARROWPHASE = 1 << 3, OVF_CONTACT_MATCH = 1 << 6, OVF_EPA_HORIZON = 1 << 8, OVF_ITERATIONS = 1 << 9, OVF_LS_ITERATIONS = 1 << 10 };
 enum { BF_PLANE = 1, BF_SPHERE = 2, BF_AABB = 4, BF_OBB = 8 };
 enum { CONTACT_TYPE_CONSTRAINT = 1, CONTACT_TYPE_SENSOR = 2 };
 
@@ -256,6 +268,9 @@ cudaError_t launch_sensor(const ModelDev& m, const DataDev& d, int stages, cudaS
 cudaError_t launch_sensor_collision(const ModelDev& m, const DataDev& d, const SensorCollisionDev& c, cudaStream_t s);
 size_t smem_sensor_collision(const SensorCollisionDev& c);
 cudaError_t launch_contact_force(const ModelDev& m, const DataDev& d, const int* contact_ids, int n, int to_world, float* out, cudaStream_t s);
+// the <contact> sensors of d's world range, after the acceleration-stage sensors (k_sensor_contact.cu)
+cudaError_t launch_sensor_contact(const ModelDev& m, const DataDev& d, const SensorContactDev& c, cudaStream_t s);
+size_t smem_sensor_contact(const SensorContactDev& c);
 // inverse dynamics at the given d.qacc into qfrc_inverse (nworld, nv); disc: d.qacc is a discrete-time acceleration, converted first,
 // and the continuous one goes to qacc_cont (nworld, nv) (k_inverse.cu)
 cudaError_t launch_inverse(const ModelDev& m, const DataDev& d, float* qfrc_inverse, float* qacc_cont, bool disc, cudaStream_t s, const FluidDev& f);

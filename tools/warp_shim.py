@@ -251,6 +251,7 @@ def _build_warp():
 
   wp.normalize = normalize
   wp.cw_mul = lambda a, b: a._new([p * q for p, q in zip(a.v, b.v)])
+  wp.cw_div = lambda a, b: a._new([_wp_div(p, q) for p, q in zip(a.v, b.v)])
   wp.sqrt, wp.sin, wp.cos, wp.atan2, wp.acos, wp.exp, wp.log, wp.pow = _m.sqrt, _m.sin, _m.cos, _m.atan2, _m.acos, _m.exp, _m.log, _m.pow
   wp.tan = _m.tan  # render_util.py compute_ray
   wp.sign = lambda x: x._new([-1.0 if a < 0 else 1.0 for a in x.v]) if isinstance(x, Vec) else (-1.0 if x < 0 else 1.0)  # warp: sign(0) = +1
