@@ -248,6 +248,11 @@ int mjb_step_profile(const mjbModel* m, mjbData* d, void* stream, float* ms_out)
  * springs / tendons, 2 with fluid forces; k_position: 0). */
 int mjb_team_residency(const mjbModel* m, const mjbData* d, int* position_worlds, int* velocity_worlds, int* shapes);
 
+/* name of the collision kernel m's collision stage launches: "k_collision" (no mesh geoms), "k_collision_mesh", or "k_collision_mesh_large"
+ * (a hull polygon of more than 32 vertices or a hull vertex in more than 16 polygons: model-sized multi-contact buffers in global scratch,
+ * and the collision sensors' kernel built the same way); null with mjb_last_error set if m is not finalized */
+const char* mjb_collision_kernel(const mjbModel* m);
+
 /* number of kernels launched by the calling thread's last mjb_* call that enqueues work, counted at each launch (memsets are not
  * kernels and are not counted); bench.py's gpu_launches */
 int mjb_last_launch_count(void);

@@ -12,7 +12,7 @@ from . import scenes
 from ._src import mjcf
 from ._src._lib import build
 from ._src.forward import camlight, collision, com_pos, crb, ctrl_noise, euler, factor_m, forward, fwd_acceleration, fwd_actuation
-from ._src.forward import fwd_position, fwd_velocity, kinematics, last_launch_count, make_constraint, solve, step, step_profile, team_residency, transmission
+from ._src.forward import collision_kernel, fwd_position, fwd_velocity, kinematics, last_launch_count, make_constraint, solve, step, step_profile, team_residency, transmission
 from ._src.forward import energy_pos, energy_vel
 from ._src.forward import com_vel, contact_force, fwd_kinematics, get_state, implicit, mul_m, passive, rne, rungekutta4, sensor_acc, sensor_pos, sensor_vel, set_state, solve_m, step1, step2
 from ._src.history import init_ctrl_history, init_sensor_history, read_ctrl, read_sensor

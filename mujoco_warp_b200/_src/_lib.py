@@ -15,7 +15,7 @@ _PKG = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 _CSRC = os.path.join(_PKG, "csrc")
 LIB_PATH = os.environ.get("MJB_LIB", os.path.join(_PKG, "libmjb200.so"))  # MJB_LIB: A/B-test an alternative build
 HEADER_PATH = os.path.join(os.path.dirname(_PKG), "include", "mjb200.h")
-SOURCES = ["capi.cu", "k_position.cu", "k_collision.cu", "k_collision_mesh.cu", "k_constraint.cu", "k_velocity.cu", "k_solver.cu", "k_integrate.cu", "k_implicit.cu", "k_support.cu", "k_sensor.cu", "k_sensor_collision.cu", "k_sensor_contact.cu", "k_ray.cu", "k_inverse.cu", "k_set_const.cu", "k_energy.cu", "k_history.cu", "k_render.cu"]
+SOURCES = ["capi.cu", "k_position.cu", "k_collision.cu", "k_collision_mesh.cu", "k_collision_mesh_large.cu", "k_constraint.cu", "k_velocity.cu", "k_solver.cu", "k_integrate.cu", "k_implicit.cu", "k_support.cu", "k_sensor.cu", "k_sensor_collision.cu", "k_sensor_collision_large.cu", "k_sensor_contact.cu", "k_ray.cu", "k_inverse.cu", "k_set_const.cu", "k_energy.cu", "k_history.cu", "k_render.cu"]
 NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a", "--extended-lambda", "-Xcompiler", "-fPIC", "-shared"]
 
 _lib = None
@@ -52,8 +52,9 @@ def build(force: bool = False, verbose: bool = False) -> str:
   os.makedirs(objdir, exist_ok=True)
   hdr_t = max(os.path.getmtime(p) for p in _headers())
   flags = [f for f in NVCC_FLAGS if f != "-shared"] + (["-Xptxas=-v"] if verbose else [])
-  # k_collision_mesh.cu includes k_collision.cu
-  extra_dep = {"k_collision_mesh.cu": [os.path.join(_CSRC, "k_collision.cu")]}
+  # the mesh builds include k_collision.cu / k_sensor_collision.cu
+  extra_dep = {"k_collision_mesh.cu": [os.path.join(_CSRC, "k_collision.cu")], "k_collision_mesh_large.cu": [os.path.join(_CSRC, "k_collision.cu")],
+               "k_sensor_collision_large.cu": [os.path.join(_CSRC, "k_sensor_collision.cu")]}
 
   def compile_one(src):
     path, obj = os.path.join(_CSRC, src), os.path.join(objdir, src[:-3] + ".o")
@@ -126,6 +127,8 @@ def lib():
     getattr(L, f).restype = ci
   L.mjb_step_profile.argtypes = [vp, vp, vp, ctypes.POINTER(ctypes.c_float)]
   L.mjb_last_launch_count.restype = ci
+  L.mjb_collision_kernel.argtypes = [vp]
+  L.mjb_collision_kernel.restype = cp
   _lib = L
   return L
 

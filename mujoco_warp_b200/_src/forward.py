@@ -301,6 +301,16 @@ def step_profile(m: Model, d: Data):
   return dict(zip(KERNEL_NAMES, [float(x) for x in out]))
 
 
+def collision_kernel(m: Model) -> str:
+  """Name of the kernel the collision stage launches for m: "k_collision" (no mesh geoms), "k_collision_mesh", or "k_collision_mesh_large"
+  (a hull polygon of more than 32 vertices or a hull vertex in more than 16 polygons: multi-contact buffers sized from the model, in global
+  scratch that make_data allocates; the collision sensors then run the same build).  Its time is step_profile()'s "collision"."""
+  name = _lib.lib().mjb_collision_kernel(m._handle)
+  if name is None:
+    _lib.check(-1)
+  return name.decode()
+
+
 TEAM_INSTANCES = ("plain", "pext", "fluid")
 
 

@@ -685,8 +685,12 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   # mesh assets (reference Model.mesh_*, types.py): vertex blocks, hull graphs for hill-climbing support queries, hull polygons
   nmesh = int(getattr(mjm, "nmesh", 0))
   m.nmesh = nmesh
-  if nmesh and (int(getattr(mjm, "npolygonmax", 0)) > 32 or int(getattr(mjm, "nmeshdegmax", 0)) > 16):
-    raise NotImplementedError(f"mesh hull with {mjm.npolygonmax} vertices in one polygon / {mjm.nmeshdegmax} polygons at one vertex: the mesh multi-contact buffers hold 32 / 16")
+  # most vertices in one hull polygon / most hull polygons at one vertex: past 32 / 16 the collision stage runs the build whose multi-contact
+  # buffers are sized from these (make_data allocates its scratch)
+  m.npolygonmax = int(getattr(mjm, "npolygonmax", 0)) if nmesh else 0
+  m.nmeshdegmax = int(getattr(mjm, "nmeshdegmax", 0)) if nmesh else 0
+  if nmesh and int(np.asarray(mjm.mesh_vertnum).max()) > 0xFFFF:
+    raise NotImplementedError(f"mesh with {int(np.asarray(mjm.mesh_vertnum).max())} vertices: the convex collision packs mesh vertex ids in 16 bits (at most 65535)")
   m.geom_dataid = dev_i(getattr(mjm, "geom_dataid", -np.ones(m.ngeom)))
   for n in ("mesh_vertadr", "mesh_vertnum", "mesh_graphadr", "mesh_graph", "mesh_polynum", "mesh_polyadr", "mesh_polyvertadr", "mesh_polyvertnum",
             "mesh_polyvert", "mesh_polymapadr", "mesh_polymapnum", "mesh_polymap"):
@@ -747,7 +751,8 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   for k, v in (("nsensorcollision", m.nsensorcollision), ("nsensorcollision_sensor", len(m.sensor_collision_id)), ("sensor_collision_epa_iterations", m.sensor_collision_epa_iterations),
                ("nsensorcollision_ccd", m.nsensorcollision_ccd), ("nsensor_energy", len(t["sensor_energy_adr"])),
                ("sensor_e_potential", m.sensor_e_potential), ("sensor_e_kinetic", m.sensor_e_kinetic),
-               ("nsensorcontact", m.nsensorcontact), ("contact_sensor_maxmatch", m.opt.contact_sensor_maxmatch), ("nhistory", m.nhistory), ("nactuator_history", int((hf["actuator_history"][:, 0] > 0).sum())), ("nsensor_history", len(m.sensor_history_id))):
+               ("nsensorcontact", m.nsensorcontact), ("contact_sensor_maxmatch", m.opt.contact_sensor_maxmatch), ("nhistory", m.nhistory), ("nactuator_history", int((hf["actuator_history"][:, 0] > 0).sum())), ("nsensor_history", len(m.sensor_history_id)),
+               ("npolygonmax", m.npolygonmax), ("nmeshdegmax", m.nmeshdegmax)):
     _lib.check(L.mjb_model_set_int(h, k.encode(), int(v)))
   g = np.asarray(o.gravity, dtype=np.float64)
   floats = dict(timestep=o.timestep, tolerance=tol, ls_tolerance=o.ls_tolerance, impratio_invsqrt=1.0 / np.sqrt(o.impratio),

@@ -18,6 +18,7 @@ struct mjbModel {
   SetConstDev setc;  // actuator_acc0 and the meaninertia output, bound by name; qpos_save stays null here (the Data's)
   EnergyDev en;      // the energy sensors; energy stays null here (the Data's: energy() below)
   HistoryDev hist;   // the delay fields; history and ctrl_delayed stay null here (the Data's: history() below)
+  MeshClipDev mclip;  // npolygonmax / nmeshdegmax; nslot and scratch stay zero here (the Data's: mesh_clip() below)
   bool finalized;
 };
 struct mjbData {
@@ -37,6 +38,8 @@ struct mjbData {
   float* energy;        // Data.energy, (nworld, 2), bound by name; passed to k_energy in EnergyDev
   float* history;       // Data.history, (nworld, nhistory), bound by name; passed to k_history in HistoryDev
   float* ctrl_delayed;  // (nworld, nu) the delayed ctrl the actuation stage reads; allocated for models with actuator delays only
+  int mclip_nslot;      // slices per world of mclip_scratch
+  float* mclip_scratch;  // the mesh multi-contact scratch (MeshClipDev); allocated for models past the fixed buffers only
 };
 
 namespace {
@@ -55,6 +58,14 @@ static FluidDev fluid(const mjbModel* m, const mjbData* d) { FluidDev f = m->flu
 static EnergyDev energy(const mjbModel* m, const mjbData* d) { EnergyDev e = m->en; e.energy = d->energy; return e; }
 // The delay fields of a model bound to a Data's history buffers
 static HistoryDev history(const mjbModel* m, const mjbData* d) { HistoryDev h = m->hist; h.history = d->history; h.ctrl_delayed = d->ctrl_delayed; return h; }
+// The mesh multi-contact sizes of a model bound to a Data's scratch; models with such hulls run the CCD_MESH = 2 kernels
+static MeshClipDev mesh_clip(const mjbModel* m, const mjbData* d) { MeshClipDev c = m->mclip; c.nslot = d->mclip_nslot; c.scratch = d->mclip_scratch; return c; }
+static bool mesh_large(const mjbModel* m) { return m->dev.nmesh > 0 && mesh_clip_large(m->mclip.npolygonmax, m->mclip.nmeshdegmax); }
+// scratch slices per world: k_collision's GJK / EPA lanes (4), or the collision-sensor kernel's EPA slots when it has more
+static int mesh_clip_slots(const mjbModel* m) { return std::max(4, std::min(32, m->sc.nsensorcollision_ccd)); }
+static cudaError_t collision(const mjbModel* m, const mjbData* d, const DataDev& dd, cudaStream_t s) {
+  return mesh_large(m) ? launch_collision_mesh_large(m->dev, dd, mesh_clip(m, d), s) : launch_collision(m->dev, dd, s);
+}
 
 extern "C" {
 
@@ -71,6 +82,7 @@ mjbModel* mjb_model_create(void) {
   memset(&m->setc, 0, sizeof(SetConstDev));
   memset(&m->en, 0, sizeof(EnergyDev));
   memset(&m->hist, 0, sizeof(HistoryDev));
+  memset(&m->mclip, 0, sizeof(MeshClipDev));
   m->finalized = false;
   return m;
 }
@@ -100,6 +112,9 @@ int mjb_model_set_int(mjbModel* m, const char* name, int v) {
 #undef X
 #define X(n) if (!strcmp(name, #n)) { m->hist.n = v; return 0; }
   MJB_HISTORY_INTS(X)
+#undef X
+#define X(n) if (!strcmp(name, #n)) { m->mclip.n = v; return 0; }
+  MJB_MESHCLIP_INTS(X)
 #undef X
   return fail(std::string("unknown model int field: ") + name);
 }
@@ -203,6 +218,8 @@ mjbData* mjb_data_create(int nworld, int nconmax, int naconmax, int njmax, int n
   d->energy = nullptr;
   d->history = nullptr;
   d->ctrl_delayed = nullptr;
+  d->mclip_nslot = 0;
+  d->mclip_scratch = nullptr;
   return d;
 }
 void mjb_data_destroy(mjbData* d) {
@@ -214,6 +231,7 @@ void mjb_data_destroy(mjbData* d) {
   if (d->rk) cudaFree(d->rk);
   if (d->qpos_save) cudaFree(d->qpos_save);
   if (d->ctrl_delayed) cudaFree(d->ctrl_delayed);
+  if (d->mclip_scratch) cudaFree(d->mclip_scratch);
   if (d->nsplit > 1) {
     for (int i = 0; i < d->nsplit; i++) { cudaStreamDestroy(d->aux[i]); cudaEventDestroy(d->ev_join[i]); }
     cudaEventDestroy(d->ev_fork);
@@ -277,6 +295,18 @@ int mjb_data_finalize(mjbData* d, const mjbModel* m) {
              smem_sensor_collision(m->sc), kMaxSmem);
     return fail(buf);
   }
+  if (mesh_large(m) && !d->mclip_scratch) {
+    d->mclip_nslot = mesh_clip_slots(m);
+    const size_t bytes = sizeof(float) * (size_t)d->dev.nworld * (size_t)d->mclip_nslot * (size_t)mesh_clip_words(m->mclip);
+    if (cudaMalloc(&d->mclip_scratch, bytes) != cudaSuccess) {
+      cudaGetLastError();
+      d->mclip_scratch = nullptr;
+      char buf[240];
+      snprintf(buf, sizeof buf, "collision kernel needs %zu B of global scratch for the mesh multi-contact (%d worlds x %d slices x %d floats; npolygonmax %d, nmeshdegmax %d)",
+               bytes, d->dev.nworld, d->mclip_nslot, mesh_clip_words(m->mclip), m->mclip.npolygonmax, m->mclip.nmeshdegmax);
+      return fail(buf);
+    }
+  }
   {
     const char* e = getenv("MJB_SPLIT");
     const int want = e ? atoi(e) : 2;
@@ -323,7 +353,7 @@ int mjb_com_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_
 int mjb_camlight(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_CAMLIGHT, s)); return 0; }
 int mjb_crb(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_CRB, s)); return 0; }
 int mjb_transmission(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_position(m->dev, d->dev, STG_TRANSMISSION, s)); return 0; }
-int mjb_collision(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(reset_contact_counters(d->dev, s)); MJB_LAUNCH(launch_collision(m->dev, d->dev, s)); return 0; }
+int mjb_collision(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(reset_contact_counters(d->dev, s)); MJB_LAUNCH(collision(m, d, d->dev, s)); return 0; }
 int mjb_make_constraint(const mjbModel* m, mjbData* d, void* stream) {
   MJB_ENTER();
   MJB_LAUNCH(launch_constraint(m->dev, d->dev, s));
@@ -415,8 +445,16 @@ int mjb_render_rays(const mjbRender* rc, float* ray, void* stream) {
 // The sensors of `stages` (1 pos, 2 vel, 4 acc) for dd's world range: k_sensor (with the collision sensors for the position stage), then
 // for the acceleration stage the <contact> sensors (sensor.py:2605-2658), which read the solver's efc_force.  A model without contact
 // sensors launches what it launched before they existed.
-static cudaError_t sensors(const mjbModel* m, const DataDev& dd, int stages, cudaStream_t s) {
-  const cudaError_t e = launch_sensor(m->dev, dd, stages, s, m->sc);
+static cudaError_t sensors(const mjbModel* m, const mjbData* d, const DataDev& dd, int stages, cudaStream_t s) {
+  cudaError_t e;
+  if (mesh_large(m) && m->sc.nsensorcollision > 0) {  // the collision sensors run the CCD_MESH = 2 build, after k_sensor as launch_sensor orders them
+    SensorCollisionDev none = m->sc;
+    none.nsensorcollision = 0;
+    e = launch_sensor(m->dev, dd, stages, s, none);
+    if (e == cudaSuccess && m->dev.nsensor > 0 && (stages & 1) && !(m->dev.disableflags & DSBL_SENSOR)) e = launch_sensor_collision_large(m->dev, dd, m->sc, mesh_clip(m, d), s);
+  } else {
+    e = launch_sensor(m->dev, dd, stages, s, m->sc);
+  }
   if (e != cudaSuccess || m->dev.nsensor == 0 || !(stages & 4) || m->scon.nsensorcontact == 0 || (m->dev.disableflags & DSBL_SENSOR)) return e;
   return launch_sensor_contact(m->dev, dd, m->scon, s);
 }
@@ -436,7 +474,7 @@ static int energy_forward_parts(const mjbModel* m) {
 
 int mjb_sensor_pos(const mjbModel* m, mjbData* d, void* stream) {
   MJB_ENTER();
-  MJB_LAUNCH(sensors(m, d->dev, 1, s));
+  MJB_LAUNCH(sensors(m, d, d->dev, 1, s));
   MJB_LAUNCH(launch_energy(m->dev, d->dev, energy(m, d), energy_sensor_parts(m), s));
   MJB_LAUNCH(history_sensor(m, d, d->dev, 1, s));
   return 0;
@@ -445,13 +483,13 @@ int mjb_energy_pos(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); M
 int mjb_energy_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_energy(m->dev, d->dev, energy(m, d), ENERGY_KIN, s)); return 0; }
 int mjb_sensor_vel(const mjbModel* m, mjbData* d, void* stream) {
   MJB_ENTER();
-  MJB_LAUNCH(sensors(m, d->dev, 2, s));
+  MJB_LAUNCH(sensors(m, d, d->dev, 2, s));
   MJB_LAUNCH(history_sensor(m, d, d->dev, 2, s));
   return 0;
 }
 int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream) {
   MJB_ENTER();
-  MJB_LAUNCH(sensors(m, d->dev, 4, s));
+  MJB_LAUNCH(sensors(m, d, d->dev, 4, s));
   MJB_LAUNCH(history_sensor(m, d, d->dev, 4, s));
   return 0;
 }
@@ -481,7 +519,7 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
     // forward.py:635-677 with factorize=False: kinematics, com_pos, camlight, crb, collision, make_constraint, transmission
     MJB_LAUNCH(launch_position(m->dev, dd, STG_KINEMATICS | STG_COM_POS | STG_CAMLIGHT | STG_CRB | STG_TRANSMISSION, s));
     MJB_MARK(0);
-    MJB_LAUNCH(launch_collision(m->dev, dd, s));
+    MJB_LAUNCH(collision(m, d, dd, s));
     MJB_MARK(1);
     MJB_LAUNCH(launch_constraint(m->dev, dd, s));
     if (dd.njmax_nnz > 0) MJB_LAUNCH(launch_efc_csr(m->dev, dd, s));  // sparse models: the reference's CSR arrays next to the dense rows
@@ -496,7 +534,7 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
   if (what & RUN_SOLVER) {
     MJB_LAUNCH(launch_solver(m->dev, dd, s));
     // sensors of all three stages in one launch after the solver (forward.py:1350-1365 interleaves them; their inputs are final by now)
-    if (m->dev.nsensor > 0) MJB_LAUNCH(sensors(m, dd, 7, s));
+    if (m->dev.nsensor > 0) MJB_LAUNCH(sensors(m, d, dd, 7, s));
     // energy after the sensors (the reference's energy_pos / energy_vel, forward.py:1327-1356): its inputs are final since fwd_velocity
     MJB_LAUNCH(launch_energy(m->dev, dd, energy(m, d), energy_forward_parts(m), s));
     MJB_LAUNCH(history_sensor(m, d, dd, 7, s));  // after every kernel that writes sensordata
@@ -510,7 +548,7 @@ static int chain(const mjbModel* m, const mjbData* d, const DataDev& dd, int wha
     if (m->dev.nsensor > 0) {
       DataDev ds = dd;
       if (disc) ds.qacc = d->inv_qacc;
-      MJB_LAUNCH(sensors(m, ds, 7, s));
+      MJB_LAUNCH(sensors(m, d, ds, 7, s));
     }
     MJB_LAUNCH(launch_energy(m->dev, dd, energy(m, d), energy_sensor_parts(m), s));  // inverse computes energy only for its sensors
     MJB_LAUNCH(history_sensor(m, d, dd, 7, s));
@@ -589,6 +627,11 @@ int mjb_step_profile(const mjbModel* m, mjbData* d, void* stream, float* ms_out)
   for (int i = 0; i < 6 && !rc; i++) rc = check(cudaEventElapsedTime(&ms_out[i], ev[i], ev[i + 1]), "cudaEventElapsedTime");
   for (int i = 0; i < n; i++) cudaEventDestroy(ev[i]);
   return rc;
+}
+const char* mjb_collision_kernel(const mjbModel* m) {
+  if (!m || !m->finalized) { fail("model not finalized"); return nullptr; }
+  if (m->dev.nmesh == 0) return "k_collision";
+  return mesh_large(m) ? "k_collision_mesh_large" : "k_collision_mesh";
 }
 int mjb_team_residency(const mjbModel* m, const mjbData* d, int* position_worlds, int* velocity_worlds, int* shapes) {
   if (!m || !d || !m->finalized || !d->finalized) return fail("model/data not finalized");

@@ -30,6 +30,15 @@ __host__ __device__ inline int surv_cap(const ModelDev& m) { return m.nxn_npair 
 
 constexpr int CCD_LANES = 4;  // geom pairs that run GJK / EPA concurrently in one warp (each needs a polytope in shared memory)
 
+// the CCD_MESH = 2 build (k_collision_mesh_large.cu) is its own kernel, with the multi-contact scratch as one more argument
+#ifdef MJB_COLLISION_MESH_LARGE_TU
+#define COL_KERNEL k_collision_mesh_large
+#define COL_EXTRA_PARAM , const __grid_constant__ MeshClipDev clipdev
+#else
+#define COL_KERNEL k_collision
+#define COL_EXTRA_PARAM
+#endif
+
 struct ColLayout { int gxpos, gxmat, surv, stage, sgeom, ccd, sap, bar, total; };
 __host__ __device__ inline ColLayout col_layout(const ModelDev& m, const DataDev& d) {
   ColLayout L;
@@ -144,7 +153,7 @@ __device__ void contact_params(const ModelDev& m, int g1, int g2, int pairid, Co
 // 8 once boxes, cylinders or ellipsoids are present.
 template <int MAXC, bool BAT>
 __global__ void __launch_bounds__(64, MAXC == 2 ? 16 : 8)
-k_collision(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d) {
+COL_KERNEL(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d COL_EXTRA_PARAM) {
   extern __shared__ float smem[];
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;  // every warp of the block owns one world (its own shared-memory slice)
   const int w = blockIdx.x * (blockDim.x >> 5) + warp + d.w0;
@@ -282,7 +291,10 @@ k_collision(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev
             fill_mesh(m, g1, a); fill_mesh(m, g2, b);
 #endif
             bool eovf = false;
-            const int nc = ccd_pair(m.ccd_tolerance, gap, m.ccd_iterations, m.epa_iterations, a, b, ccd_scratch + slot * sw, &dist, w1, w2, &eovf);
+#if CCD_MESH == 2
+            const CcdClip mc = {clipdev.scratch + ((size_t)w * clipdev.nslot + slot) * mesh_clip_words(clipdev), mesh_clip_poly(clipdev), mesh_clip_deg(clipdev)};
+#endif
+            const int nc = ccd_pair(m.ccd_tolerance, gap, m.ccd_iterations, m.epa_iterations, a, b, ccd_scratch + slot * sw, &dist, w1, w2, &eovf CCD_CLIP_ARG);
             if (eovf) ovf |= OVF_EPA_HORIZON;
             if (nc > 0 && dist < gap) {  // collision_convex.py:860-868, 935-943
               dist += margin;
@@ -477,6 +489,15 @@ k_collision(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev
 // warps (= worlds) per block: one-warp blocks cap an SM at 32 resident worlds (CTA limit)
 constexpr int collision_wpb() { return 2; }
 
+#ifdef MJB_COLLISION_MESH_LARGE_TU
+cudaError_t launch_collision_mesh_large(const ModelDev& m, const DataDev& d, const MeshClipDev& c, cudaStream_t s) {
+  static_assert(CCD_LANES <= 4, "mjb_data_finalize allocates at least 4 scratch slices per world");
+  void (*kern)(ModelDev, DataDev, MeshClipDev) = m.batched ? k_collision_mesh_large<8, true> : k_collision_mesh_large<8, false>;
+  const int grid = (d.wn + collision_wpb() - 1) / collision_wpb();
+  return launch(kern, grid, collision_wpb() * 32, (size_t)col_layout(m, d).total * sizeof(float) * collision_wpb(), s, m, d, c);
+}
+#else
+
 #ifdef MJB_COLLISION_MESH_TU
 #define LAUNCH_NAME launch_collision_mesh
 #define SMEM_NAME smem_collision_mesh
@@ -512,3 +533,4 @@ cudaError_t LAUNCH_NAME(const ModelDev& m, const DataDev& d, cudaStream_t s) {
   const int grid = (d.wn + collision_wpb() - 1) / collision_wpb();
   return launch(kern, grid, collision_wpb() * 32, SMEM_NAME(m, d), s, m, d);
 }
+#endif

@@ -27,10 +27,27 @@
 // CCD_MESH = 1 adds mesh geoms (hull-vertex support function with a cached start vertex, mesh multi-contact).  The product library carries
 // both builds of the collision kernel: k_collision.cu without it (models without mesh geoms keep the lean box / analytic code and its small
 // stack), k_collision_mesh.cu with it; tests/host_harness also builds this header with it on the host.
+// CCD_MESH = 2 is the same mesh code for hulls past the fixed buffers of CCD_MESH = 1 (npolygonmax > 32 or nmeshdegmax > 16): the multi-contact
+// buffers are a per-lane slice of scratch the caller passes in (CcdClip), sized from the model at run time, so no per-lane array grows with the
+// model (k_collision_mesh_large.cu, k_sensor_collision_large.cu).
 #ifndef CCD_MESH
 #define CCD_MESH 0
 #endif
-#if CCD_MESH
+#if CCD_MESH == 2
+#define CCD_VSHIFT 16
+#define CCD_VMASK 0xFFFF
+#define CCD_FLOAT_MIN -1e30f
+#define CCD_DEGREES(n) (n)          // the candidate buffers hold every polygon at a vertex
+#define CCD_POLY_FITS(n) true       // and every hull polygon
+#define CCD_QUAD_GUARD(np) (np)     // a walk around a polygon of np vertices takes at most np steps
+#define CCD_CLIPCAP clipcap         // twice the largest polygon (collision_convex.py:1229-1236)
+#define CCD_CLIPCAP_PARAM , int clipcap
+#define CCD_CLIPCAP_ARG , clipcap
+#define CCD_CLIP_PARAM , CcdClip mc
+#define CCD_CLIP_ARG , mc
+// one lane's multi-contact scratch: buf holds mesh_clip_words(maxpoly, maxdeg) floats (mjb_types.cuh)
+struct CcdClip { float* buf; int maxpoly, maxdeg; };
+#elif CCD_MESH
 #define CCD_VSHIFT 16        // support-vertex ids of the two geoms packed in one word: mesh vertex ids need 16 bits each
 #define CCD_VMASK 0xFFFF
 #define CCD_MAXDEG 16        // hull polygons meeting at one mesh vertex (model nmeshdegmax)
@@ -43,6 +60,15 @@
 #define CCD_MAXDEG 3
 #define CCD_MAXPOLY 4
 #define CCD_CLIPCAP 8
+#endif
+#if CCD_MESH != 2
+#define CCD_DEGREES(n) min(n, CCD_MAXDEG)
+#define CCD_POLY_FITS(n) ((n) <= CCD_MAXPOLY)
+#define CCD_QUAD_GUARD(np) 64
+#define CCD_CLIPCAP_PARAM
+#define CCD_CLIPCAP_ARG
+#define CCD_CLIP_PARAM
+#define CCD_CLIP_ARG
 #endif
 
 // Geom-type pairs the reference routes to the convex path (collision_driver.py:47-81), analytic geoms only, in table order.
@@ -617,16 +643,16 @@ static __device__ void polygon_quad(const float* poly, int np, int* res) {  // :
   res[0] = 0; res[1] = b; res[2] = c; res[3] = d;
   float m = area4(ld3(poly), ld3(poly + 3 * b), ld3(poly + 3 * c), ld3(poly + 3 * d));
   for (int a = 0; a < np; a++) {
-    for (int guard = 0; guard < 64; guard++) {
+    for (int guard = 0; guard < CCD_QUAD_GUARD(np); guard++) {
       float mn = area4(ld3(poly + 3 * a), ld3(poly + 3 * b), ld3(poly + 3 * c), ld3(poly + 3 * ((d + 1) % np)));
       if (mn <= m) break;
       m = mn; d = (d + 1) % np; res[0] = a; res[1] = b; res[2] = c; res[3] = d;
-      for (int g2 = 0; g2 < 64; g2++) {
+      for (int g2 = 0; g2 < CCD_QUAD_GUARD(np); g2++) {
         mn = area4(ld3(poly + 3 * a), ld3(poly + 3 * b), ld3(poly + 3 * ((c + 1) % np)), ld3(poly + 3 * d));
         if (mn <= m) break;
         m = mn; c = (c + 1) % np; res[0] = a; res[1] = b; res[2] = c; res[3] = d;
       }
-      for (int g3 = 0; g3 < 64; g3++) {
+      for (int g3 = 0; g3 < CCD_QUAD_GUARD(np); g3++) {
         mn = area4(ld3(poly + 3 * a), ld3(poly + 3 * ((b + 1) % np)), ld3(poly + 3 * c), ld3(poly + 3 * d));
         if (mn <= m) break;
         m = mn; b = (b + 1) % np; res[0] = a; res[1] = b; res[2] = c; res[3] = d;
@@ -636,8 +662,8 @@ static __device__ void polygon_quad(const float* poly, int np, int* res) {  // :
   }
 }
 // :1941 clip polygon face2 against the side planes of face1 (extruded along n).  witness2 lies on the clipped polygon,
-// witness1 = witness2 - dir.  buf: 48 words (two 8-vertex polygons).
-static __device__ int polygon_clip(const v3* face1, int nface1, const v3* face2, int nface2, v3 n, v3 dir, float* buf, v3* w1, v3* w2) {
+// witness1 = witness2 - dir.  buf: two polygons of CCD_CLIPCAP vertices.
+static __device__ int polygon_clip(const v3* face1, int nface1, const v3* face2, int nface2, v3 n, v3 dir, float* buf, v3* w1, v3* w2 CCD_CLIPCAP_PARAM) {
   if (nface1 < 3) return 0;
   float* poly = buf;
   float* clip = buf + 3 * CCD_CLIPCAP;
@@ -713,7 +739,7 @@ static __device__ int mesh_normals(const BoxFeat& f, const CGeom& g, v3* nout, i
     return n;
   }
   if (f.dim == 1) {
-    const int n = min(n1, CCD_MAXDEG);
+    const int n = CCD_DEGREES(n1);
     for (int i = 0; i < n; i++) { nout[i] = matvec(g.rot, ld3(g.polynormal + 3 * m1[i])); iout[i] = m1[i]; }
     return n;
   }
@@ -725,7 +751,7 @@ static __device__ int mesh_edge_normals(const BoxFeat& f, const CGeom& g, v3* no
   if (f.dim == 1) {
     const int v1i = f.idx[0];
     const int* m1 = g.polymap + g.polymapadr[v1i];
-    const int n = min(g.polymapnum[v1i], CCD_MAXDEG);
+    const int n = CCD_DEGREES(g.polymapnum[v1i]);
     for (int i = 0; i < n; i++) {
       const int adr = g.polyvertadr[m1[i]], nvert = g.polyvertnum[m1[i]];
       for (int j = 0; j < nvert; j++)
@@ -742,7 +768,7 @@ static __device__ int mesh_edge_normals(const BoxFeat& f, const CGeom& g, v3* no
 // :1891-1912 a hull polygon in world coordinates, vertex order reversed
 static __device__ int mesh_face(const CGeom& g, int idx, v3* face) {
   const int adr = g.polyvertadr[idx], nvert = g.polyvertnum[idx];
-  if (nvert > CCD_MAXPOLY) return 0;
+  if (!CCD_POLY_FITS(nvert)) return 0;
   int j = 0;
   for (int i = nvert - 1; i >= 0; i--, j++) face[j] = matvec(g.rot, ld3(g.vert + 3 * g.polyvert[adr + i])) + g.pos;
   return nvert;
@@ -755,9 +781,14 @@ static __device__ int mesh_face(const CGeom& g, int idx, v3* face) {
 #define CCD_EDGE_NORMALS(f, g, n, ev) box_edge_normals(f, g, n, ev)
 #define CCD_FACE(g, idx, face) box_face(g, idx, face)
 #endif
+#if CCD_MESH == 2
+#define CCD_MC_BUF const CcdClip& mc
+#else
+#define CCD_MC_BUF float* buf
+#endif
 // :2076 for two boxes (CCD_MESH: boxes and meshes).  Overwrites the witness arrays (4 each) and returns the contact count; buf must not alias
 // pt.vert / pt.vidx.
-static __device__ int ccd_multicontact(const Polytope& pt, int epa_face, const CGeom& g1, const CGeom& g2, float* buf, v3* w1, v3* w2) {
+static __device__ int ccd_multicontact(const Polytope& pt, int epa_face, const CGeom& g1, const CGeom& g2, CCD_MC_BUF, v3* w1, v3* w2) {
   const v3 x1 = w1[0], x2 = w2[0];
   for (int k = 1; k < 4; k++) w1[k] = w2[k] = mk3(0.f, 0.f, 0.f);
   const unsigned fw = pt.face[epa_face];
@@ -765,6 +796,14 @@ static __device__ int ccd_multicontact(const Polytope& pt, int epa_face, const C
   const BoxFeat f1 = feature_dim(pt, face, 0), f2 = feature_dim(pt, face, 1);
   const v3 ev1 = ld3(pt.vert + 6 * face[0]), ev2 = ld3(pt.vert + 6 * face[0] + 3);
   const v3 dir = x2 - x1;
+#if CCD_MESH == 2
+  // the buffers in the lane's scratch, in mesh_clip_words order; maxdeg / maxpoly are the model's, at least a box's 3 / 4
+  const int maxdeg = mc.maxdeg, clipcap = 2 * mc.maxpoly;
+  v3 *n1 = reinterpret_cast<v3*>(mc.buf), *n2 = n1 + maxdeg, *endvert = n2 + maxdeg, *face1 = endvert + maxdeg, *face2 = face1 + mc.maxpoly;
+  int *idx1 = reinterpret_cast<int*>(face2 + mc.maxpoly), *idx2 = idx1 + maxdeg;
+  float* buf = reinterpret_cast<float*>(idx2 + maxdeg);
+  for (int k = 0; k < maxdeg; k++) { idx1[k] = idx2[k] = 0; n1[k] = n2[k] = endvert[k] = mk3(0.f, 0.f, 0.f); }
+#else
   v3 n1[CCD_MAXDEG], n2[CCD_MAXDEG], endvert[CCD_MAXDEG];
 #if CCD_MESH
   int idx1[CCD_MAXDEG], idx2[CCD_MAXDEG];
@@ -773,6 +812,7 @@ static __device__ int ccd_multicontact(const Polytope& pt, int epa_face, const C
   int idx1[3] = {0, 0, 0}, idx2[3] = {0, 0, 0};
 #endif
   for (int k = 0; k < CCD_MAXDEG; k++) n1[k] = n2[k] = endvert[k] = mk3(0.f, 0.f, 0.f);
+#endif
   int nn1 = CCD_NORMALS(f1, g1, dir * -1.0f, n1, idx1), nn2 = CCD_NORMALS(f2, g2, dir, n2, idx2);
   bool edge1 = false, edge2 = false, found = false;
   int ri = 0, rj = 0;
@@ -790,19 +830,21 @@ static __device__ int ccd_multicontact(const Polytope& pt, int epa_face, const C
       edge2 = true;
     } else return 1;
   }
+#if CCD_MESH != 2
   v3 face1[CCD_MAXPOLY], face2[CCD_MAXPOLY];
+#endif
   int nface1, nface2;
   if (edge1) { face1[0] = ev1; face1[1] = endvert[ri]; nface1 = 2; } else nface1 = CCD_FACE(g1, edge2 ? idx1[rj] : idx1[ri], face1);
   if (edge2) { face2[0] = ev2; face2[1] = endvert[ri]; nface2 = 2; } else nface2 = CCD_FACE(g2, idx2[rj], face2);
   const float dl = length(dir);
-  if (edge1) return polygon_clip(face2, nface2, face1, nface1, n2[rj], n2[rj] * -dl, buf, w2, w1);  // roles flipped, witnesses flipped back
-  if (edge2) return polygon_clip(face1, nface1, face2, nface2, n1[rj], n1[rj] * -dl, buf, w1, w2);
-  return polygon_clip(face1, nface1, face2, nface2, n1[ri], n2[rj] * dl, buf, w1, w2);
+  if (edge1) return polygon_clip(face2, nface2, face1, nface1, n2[rj], n2[rj] * -dl, buf, w2, w1 CCD_CLIPCAP_ARG);  // roles flipped, witnesses flipped back
+  if (edge2) return polygon_clip(face1, nface1, face2, nface2, n1[rj], n1[rj] * -dl, buf, w1, w2 CCD_CLIPCAP_ARG);
+  return polygon_clip(face1, nface1, face2, nface2, n1[ri], n2[rj] * dl, buf, w1, w2 CCD_CLIPCAP_ARG);
 }
 
 // gjk_phase (:2350) + epa_phase (:2421) + multicontact for box pairs.  Returns the number of contacts (0..4, witnesses in
-// w1 / w2, 4 each); *dist is relative to the margin-inflated shapes.
-static __device__ __noinline__ int ccd_pair(float tolerance, float cutoff, int gjk_iterations, int epa_iterations, CGeom g1, CGeom g2, float* scratch, float* dist, v3* w1, v3* w2, bool* ovf) {
+// w1 / w2, 4 each); *dist is relative to the margin-inflated shapes.  CCD_MESH = 2: mc is the lane's multi-contact scratch.
+static __device__ __noinline__ int ccd_pair(float tolerance, float cutoff, int gjk_iterations, int epa_iterations, CGeom g1, CGeom g2, float* scratch, float* dist, v3* w1, v3* w2, bool* ovf CCD_CLIP_PARAM) {
   const CGeom o1 = g1, o2 = g2;
   float full1 = 0.f, full2 = 0.f, size1 = 0.f, size2 = 0.f;
 #if CCD_MESH
@@ -851,7 +893,9 @@ static __device__ __noinline__ int ccd_pair(float tolerance, float cutoff, int g
   if (pt.status) { *dist = r.dist; w1[0] = r.x1; w2[0] = r.x2; return 1; }
   const int fidx = ccd_epa(tolerance, epa_iterations, pt, g1, g2, boxes, dist, &w1[0], &w2[0], ovf);
   if (fidx == -1) { *dist = CCD_FLOAT_MAX; return 0; }
-#if CCD_MESH
+#if CCD_MESH == 2
+  if (boxes && (g1.type != GEOM_MESH || g1.polynum > 0) && (g2.type != GEOM_MESH || g2.polynum > 0)) return ccd_multicontact(pt, fidx, g1, g2, mc, w1, w2);
+#elif CCD_MESH
   if (boxes && (g1.type != GEOM_MESH || g1.polynum > 0) && (g2.type != GEOM_MESH || g2.polynum > 0)) {  // a mesh without polygon data keeps one contact
     float clipbuf[2 * 3 * CCD_CLIPCAP];
     return ccd_multicontact(pt, fidx, g1, g2, clipbuf, w1, w2);

@@ -5,7 +5,7 @@
 // _sensor_collision (the witness points pos -/+ 0.5 dist normal) and sensor.py:642-718 (the reduction, flip and cutoff rules).  Every pair
 // runs the collider the reference routes its geom types to and reports every contact that collider writes; nothing reaches the contact pool.
 //
-// Scalar code, one geom pair or one sensor per thread.  Needs the CCD_MESH build of mjb_ccd.cuh.
+// Scalar code, one geom pair or one sensor per thread.  Needs the CCD_MESH build of mjb_ccd.cuh (1, or 2 with the lane's multi-contact scratch).
 #pragma once
 #include "mjb_ccd.cuh"
 #include "mjb_colliders.cuh"
@@ -20,7 +20,7 @@ constexpr int SC_PAIR_WORDS = 4;  // sensor_collision_pair row: geom1, geom2, ex
 // its witness points pos -/+ 0.5 dist normal.  scratch: ccd_scratch_words(epa_iterations) floats for EPA.  Returns whether EPA ran out
 // of horizon edges (OVF_EPA_HORIZON, as k_collision reports it).
 static __device__ bool sensor_pair(const ModelDev& m, const float* gxpos, const float* gxmat, int g1, int g2, int pid, int epa_iterations, float* scratch,
-                                   float* out) {
+                                   float* out CCD_CLIP_PARAM) {
   float cd[8];
   v3 cp[8], cn[8];
   for (int k = 0; k < 8; k++) { cd[k] = INFINITY; cp[k] = mk3(0.f, 0.f, 0.f); cn[k] = mk3(1.f, 0.f, 0.f); }
@@ -77,7 +77,7 @@ static __device__ bool sensor_pair(const ModelDev& m, const float* gxpos, const 
     float dist = 0.f;
     v3 w1[4], w2[4];
     w1[0] = w2[0] = mk3(0.f, 0.f, 0.f);
-    const int nc = ccd_pair(m.ccd_tolerance, 1.0e32f, m.ccd_iterations, epa_iterations, a, b, scratch, &dist, w1, w2, &eovf);
+    const int nc = ccd_pair(m.ccd_tolerance, 1.0e32f, m.ccd_iterations, epa_iterations, a, b, scratch, &dist, w1, w2, &eovf CCD_CLIP_ARG);
     dist += margin;
     const v3 nrm = dist <= margin ? w1[0] - w2[0] : w2[0] - w1[0];
     for (int k = 0; k < nc; k++) { cd[k] = dist; cp[k] = (w1[k] + w2[k]) * 0.5f; cn[k] = nrm; }

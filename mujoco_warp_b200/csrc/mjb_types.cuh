@@ -206,6 +206,27 @@ struct HistoryDev {
   float* __restrict__ ctrl_delayed;             // (nworld, nu) the ctrl k_velocity's actuation reads (mjb_data_finalize allocates it)
 };
 
+// ---------------------------------------------------------------- mesh multi-contact scratch (k_collision_mesh_large.cu, k_sensor_collision_large.cu)
+// Models whose hulls have a polygon of more than kMeshPolyCap vertices, or a vertex shared by more than kMeshDegCap polygons, run the CCD_MESH = 2
+// build of the collision and collision-sensor kernels.  Its multi-contact buffers are sized from the model and live in global scratch: nslot
+// slices per world, one per lane that runs GJK / EPA at once.  Passed as one extra argument to those kernels only, for the same reason as FluidDev.
+constexpr int kMeshPolyCap = 32, kMeshDegCap = 16;  // the fixed buffers of the CCD_MESH = 1 build (mjb_ccd.cuh)
+#define MJB_MESHCLIP_INTS(X) X(npolygonmax) X(nmeshdegmax)
+struct MeshClipDev {
+  int npolygonmax;              // Model.npolygonmax: most vertices in one hull polygon
+  int nmeshdegmax;              // Model.nmeshdegmax: most hull polygons at one vertex
+  int nslot;                    // scratch slices per world
+  float* __restrict__ scratch;  // (nworld, nslot, mesh_clip_words) allocated by mjb_data_finalize for such models only
+};
+__host__ __device__ inline bool mesh_clip_large(int npolygonmax, int nmeshdegmax) { return npolygonmax > kMeshPolyCap || nmeshdegmax > kMeshDegCap; }
+// buffer sizes: the model's, and at least a box's 4-vertex face / 3 faces at a corner
+__host__ __device__ inline int mesh_clip_poly(const MeshClipDev& c) { return c.npolygonmax > 4 ? c.npolygonmax : 4; }
+__host__ __device__ inline int mesh_clip_deg(const MeshClipDev& c) { return c.nmeshdegmax > 3 ? c.nmeshdegmax : 3; }
+// floats of one slice: candidate normals of each geom and the edge end vertices (3 maxdeg each), the polygon ids of each geom's normals (maxdeg
+// each), the two faces (3 maxpoly each) and the two clip buffers (3 x 2 maxpoly each)
+__host__ __device__ inline int mesh_clip_words(int maxpoly, int maxdeg) { return 11 * maxdeg + 18 * maxpoly; }
+__host__ __device__ inline int mesh_clip_words(const MeshClipDev& c) { return mesh_clip_words(mesh_clip_poly(c), mesh_clip_deg(c)); }
+
 // ---------------------------------------------------------------- enums (MuJoCo values; see constants.py)
 enum { JNT_FREE = 0, JNT_BALL = 1, JNT_SLIDE = 2, JNT_HINGE = 3 };
 enum { GEOM_PLANE = 0, GEOM_HFIELD, GEOM_SPHERE, GEOM_CAPSULE, GEOM_ELLIPSOID, GEOM_CYLINDER, GEOM_BOX, GEOM_MESH };
@@ -252,6 +273,8 @@ enum { STG_VELOCITY = 1, STG_ACTUATION = 2, STG_ACCELERATION = 4, STG_FACTOR_ONL
 cudaError_t launch_position(const ModelDev& m, const DataDev& d, int stage_mask, cudaStream_t s);
 cudaError_t launch_collision(const ModelDev& m, const DataDev& d, cudaStream_t s);
 cudaError_t launch_collision_mesh(const ModelDev& m, const DataDev& d, cudaStream_t s);  // CCD_MESH build of the same kernel (k_collision_mesh.cu)
+// CCD_MESH = 2 build for hulls past the fixed buffers (k_collision_mesh_large.cu); same shared memory as the CCD_MESH build
+cudaError_t launch_collision_mesh_large(const ModelDev& m, const DataDev& d, const MeshClipDev& c, cudaStream_t s);
 size_t smem_collision_mesh(const ModelDev& m, const DataDev& d);
 cudaError_t reset_contact_counters(const DataDev& d, cudaStream_t s);
 cudaError_t launch_constraint(const ModelDev& m, const DataDev& d, cudaStream_t s);
@@ -267,6 +290,7 @@ size_t smem_implicit(const ModelDev& m);
 cudaError_t launch_sensor(const ModelDev& m, const DataDev& d, int stages, cudaStream_t s, const SensorCollisionDev& c);
 cudaError_t launch_sensor_collision(const ModelDev& m, const DataDev& d, const SensorCollisionDev& c, cudaStream_t s);
 size_t smem_sensor_collision(const SensorCollisionDev& c);
+cudaError_t launch_sensor_collision_large(const ModelDev& m, const DataDev& d, const SensorCollisionDev& c, const MeshClipDev& mc, cudaStream_t s);
 cudaError_t launch_contact_force(const ModelDev& m, const DataDev& d, const int* contact_ids, int n, int to_world, float* out, cudaStream_t s);
 // the <contact> sensors of d's world range, after the acceleration-stage sensors (k_sensor_contact.cu)
 cudaError_t launch_sensor_contact(const ModelDev& m, const DataDev& d, const SensorContactDev& c, cudaStream_t s);
