@@ -46,6 +46,14 @@ _BATCHABLE_EXTRA = ("eq_solref", "eq_solimp", "eq_data", "pair_friction", "pair_
 # the renderer's float Model fields that carry the reference's `*` leading dimension (types.py cam_fovy ... mat_emission)
 _RENDER_FLOATS = ("cam_fovy", "cam_intrinsic", "light_attenuation", "light_cutoff", "light_exponent", "light_ambient", "light_diffuse", "light_specular",
                   "mat_specular", "mat_shininess", "mat_emission")
+# per-world float fields the magnetometer and camprojection sensors read (types.py opt.magnetic, cam_fovy, cam_intrinsic)
+_SENSOR_BATCHED = ("magnetic", "cam_fovy", "cam_intrinsic")
+# sensor types k_sensor runs in its EXTRA build only, with the object type each reads and its reference object's (None: none)
+_EXTRA_SENSORS = {
+  C.SENS_MAGNETOMETER: ((C.OBJ_SITE,), None), C.SENS_CAMPROJECTION: ((C.OBJ_SITE,), (C.OBJ_CAMERA,)),
+  C.SENS_INSIDESITE: ((C.OBJ_BODY, C.OBJ_XBODY, C.OBJ_GEOM, C.OBJ_SITE, C.OBJ_CAMERA), (C.OBJ_SITE,)),
+  **{t: ((C.OBJ_TENDON,), None) for t in (C.SENS_TENDONLIMITPOS, C.SENS_TENDONLIMITVEL, C.SENS_TENDONLIMITFRC, C.SENS_TENDONACTFRC)},
+}
 _SIZES = ["nq", "nv", "nu", "na", "nbody", "njnt", "ngeom", "nsite", "ncam", "nlight", "ntree", "nkey", "nmocap", "neq", "ntendon", "nflex"]
 
 _SUPPORTED_PAIRS = {
@@ -457,6 +465,32 @@ def _contact_sensor_intprm(mjm) -> np.ndarray:
   return out
 
 
+def _validate_extra_sensors(mjm):
+  """Checks the object kinds and ids of the magnetometer / camprojection / insidesite / tendon sensors again, for models that did not come
+  from this package's compiler.  Returns whether the model has one (k_sensor's EXTRA build)."""
+  ns = int(getattr(mjm, "nsensor", 0))
+  stype = np.asarray(mjm.sensor_type).reshape(ns) if ns else np.zeros(0, dtype=int)
+  counts = {C.OBJ_BODY: int(mjm.nbody), C.OBJ_XBODY: int(mjm.nbody), C.OBJ_GEOM: int(mjm.ngeom), C.OBJ_SITE: int(getattr(mjm, "nsite", 0)),
+            C.OBJ_CAMERA: int(getattr(mjm, "ncam", 0)), C.OBJ_TENDON: int(getattr(mjm, "ntendon", 0))}
+  names = getattr(getattr(mjm, "names", None), "sensor", None)
+  found = False
+  for s in range(ns):
+    if int(stype[s]) not in _EXTRA_SENSORS:
+      continue
+    found = True
+    what = f"sensor {s}" + (f" ('{names[s]}')" if names is not None and s < len(names) else "")
+    for side, kinds, typ, oid in (("object", _EXTRA_SENSORS[int(stype[s])][0], int(mjm.sensor_objtype[s]), int(mjm.sensor_objid[s])),
+                                  ("reference", _EXTRA_SENSORS[int(stype[s])][1], int(getattr(mjm, "sensor_reftype", np.zeros(ns))[s]),
+                                   int(getattr(mjm, "sensor_refid", -np.ones(ns))[s]))):
+      if kinds is None:
+        continue
+      if typ not in kinds:
+        raise ValueError(f"{what}: {side} type {typ}; expected one of {kinds}")
+      if not 0 <= oid < counts[typ]:
+        raise ValueError(f"{what}: {side} names an unknown object (id {oid})")
+  return found
+
+
 def _validate_history(mjm):
   """Refuses, by name, delays and intervals the history buffers would not honour: the reference silently reads the undelayed value
   when nsample is 0 (history.py:380), and negative sizes / times have no meaning."""
@@ -557,6 +591,8 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
     # model constants here, one value for every world (the reference indexes them per world)
     density=f32(float(getattr(o, "density", 0.0))), viscosity=f32(float(getattr(o, "viscosity", 0.0))),
     wind=f32(np.asarray(getattr(o, "wind", np.zeros(3)), dtype=np.float64).reshape(3)),
+    # (nb, 3): world w reads entry w % nb (assign an (nworld, 3) tensor for per-world fields); MuJoCo's default for older models
+    magnetic=f32(np.asarray(getattr(o, "magnetic", (0.0, -0.5, 0.0)), dtype=np.float64).reshape(3)),
   )
   if len(t["nxn_geom_pair_filtered"]) >= 250_000:
     # the reference switches to sweep-and-prune here (io.py:631-636); this build keeps one world's geoms and pair list in one
@@ -645,6 +681,7 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   m.site_size = dev_f(getattr(mjm, "site_size", np.full((nsite, 3), 0.005)), batched=False)
   stype = np.asarray(mjm.sensor_type) if nsensor else np.zeros(0, dtype=int)
   m.sensor_subtree_vel = bool(np.isin(stype, (C.SENS_SUBTREELINVEL, C.SENS_SUBTREEANGMOM)).any())  # reference io.py:896-897
+  m.sensor_extra = _validate_extra_sensors(mjm)
   m.sensor_rne_postconstraint = bool(np.isin(stype, (C.SENS_ACCELEROMETER, C.SENS_FORCE, C.SENS_TORQUE, C.SENS_FRAMELINACC, C.SENS_FRAMEANGACC)).any())  # :900
   # <contact> sensors (reference io.py:409-413, :441, :898): their ids, [dataspec, reduce, num] per sensor, and the match capacity
   sensor_intprm = _contact_sensor_intprm(mjm)
@@ -752,7 +789,7 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
                ("nsensorcollision_ccd", m.nsensorcollision_ccd), ("nsensor_energy", len(t["sensor_energy_adr"])),
                ("sensor_e_potential", m.sensor_e_potential), ("sensor_e_kinetic", m.sensor_e_kinetic),
                ("nsensorcontact", m.nsensorcontact), ("contact_sensor_maxmatch", m.opt.contact_sensor_maxmatch), ("nhistory", m.nhistory), ("nactuator_history", int((hf["actuator_history"][:, 0] > 0).sum())), ("nsensor_history", len(m.sensor_history_id)),
-               ("npolygonmax", m.npolygonmax), ("nmeshdegmax", m.nmeshdegmax)):
+               ("npolygonmax", m.npolygonmax), ("nmeshdegmax", m.nmeshdegmax), ("sensor_extra", int(m.sensor_extra))):
     _lib.check(L.mjb_model_set_int(h, k.encode(), int(v)))
   g = np.asarray(o.gravity, dtype=np.float64)
   floats = dict(timestep=o.timestep, tolerance=tol, ls_tolerance=o.ls_tolerance, impratio_invsqrt=1.0 / np.sqrt(o.impratio),
@@ -764,6 +801,7 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   dev_names = {
     "jnt_limited_adr": m.jnt_limited_slide_hinge_adr, "nxn_geom_pair": m.nxn_geom_pair_filtered, "nxn_pairid": m.nxn_pairid_filtered,
     "body_isdofancestor": m._isdofancestor_nv, "meaninertia": m.stat.meaninertia,  # set_const writes world 0's meaninertia here
+    "magnetic": m.opt.magnetic,
   }
   for n in (_FLOAT_FIELDS + _INT_FIELDS + ["body_childadr", "body_childid", "level_adr", "level_body", "M_entry_row", "mulm_rowadr", "mulm_col",
                                          "mulm_madr", "tree_qLDadr", "dof_fricloss_adr", "moment_rownnz0", "moment_rowadr0", "moment_colind0",
@@ -779,18 +817,19 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
                                          "geom_fluid", "body_fluid", "body_geomadr", "body_geomnum", "sensor_collision_start_adr", "sensor_collision_pair",
                                          "sensor_collision_id", "sensor_collision_adr", "sensor_collision_flip", "actuator_acc0", "actuator_lengthrange", "jnt_limited", "sensor_energy_adr",
                                          "actuator_history", "actuator_historyadr", "actuator_delay", "sensor_history", "sensor_historyadr", "sensor_delay",
-                                         "sensor_interval", "sensor_history_id", "sensor_contact_adr", "sensor_intprm"]
+                                         "sensor_interval", "sensor_history_id", "sensor_contact_adr", "sensor_intprm",
+                                         "cam_fovy", "cam_intrinsic", "cam_sensorsize", "cam_resolution"]
                                         + [n for n, _ in _TENDON_FLOATS]):
     dev_names.setdefault(n, getattr(m, n))
   for n, x in dev_names.items():
     x = _ptr_tensor(x)
     keep.append(x)
-    nb = int(x.shape[0]) if (n in _FLOAT_FIELDS or n in _BATCHABLE_EXTRA) and x.dim() >= 1 and x.numel() > 0 else 1
+    nb = int(x.shape[0]) if (n in _FLOAT_FIELDS or n in _BATCHABLE_EXTRA or n in _SENSOR_BATCHED) and x.dim() >= 1 and x.numel() > 0 else 1
     _lib.check(L.mjb_model_set_array_batched(h, n.encode(), x.data_ptr(), nb, int(x.numel() // max(nb, 1))))
   _lib.check(L.mjb_model_finalize(h))
   m._keep = keep
   weakref.finalize(m, L.mjb_model_destroy, h)
-  _install_model_rebind(m, L, set(dev_names) - {"jnt_limited_adr", "nxn_geom_pair", "nxn_pairid", "body_isdofancestor", "meaninertia"}, set(ints))
+  _install_model_rebind(m, L, set(dev_names) - {"jnt_limited_adr", "nxn_geom_pair", "nxn_pairid", "body_isdofancestor", "meaninertia", "magnetic"}, set(ints))
   return m
 
 
@@ -815,7 +854,7 @@ def _install_model_rebind(m: types.Model, L, arrays, ints):
   def model_hook(name, value):
     if name in arrays and name in m.__dict__:
       old = m.__dict__[name]
-      batchable = name in _FLOAT_FIELDS or name in _BATCHABLE_EXTRA
+      batchable = name in _FLOAT_FIELDS or name in _BATCHABLE_EXTRA or name in _SENSOR_BATCHED
       if batchable and isinstance(value, torch.Tensor) and value.dim() == old.dim() and value.shape[1:] == old.shape[1:] and value.shape[0] >= 1:
         # a per-world (batched) field may change its leading size: world w reads entry w % size (reference types.py:822-833)
         if value.dtype != old.dtype or value.device != old.device:
@@ -843,6 +882,15 @@ def _install_model_rebind(m: types.Model, L, arrays, ints):
       for k, v in zip((f"{name}_x", f"{name}_y", f"{name}_z"), g):
         _lib.check(L.mjb_model_set_float(h, k.encode(), float(v)))
       return value if isinstance(value, torch.Tensor) else torch.tensor([g], dtype=torch.float32, device=m.opt.__dict__[name].device)
+    if name == "magnetic":  # per world like the batched Model fields: (nb, 3), world w reads entry w % nb
+      old = m.opt.__dict__[name]
+      x = value if isinstance(value, torch.Tensor) else torch.tensor(np.asarray(value, dtype=np.float32), device=old.device)
+      x = x.to(dtype=old.dtype, device=old.device).reshape(-1, 3).contiguous()
+      if x.shape[0] < 1:
+        raise ValueError(f"opt.magnetic: expected (nb, 3) with nb >= 1, got {tuple(value.shape) if isinstance(value, torch.Tensor) else np.shape(value)}")
+      m._keep.append(x)
+      _lib.check(L.mjb_model_set_array_batched(h, b"magnetic", x.data_ptr(), int(x.shape[0]), 3))
+      return x
     if name in _OPT_INTS:
       if name == "integrator" and int(value) not in (C.INT_EULER, C.INT_IMPLICIT, C.INT_IMPLICITFAST, C.INT_RK4):
         raise NotImplementedError(f"integrator {value} not implemented")

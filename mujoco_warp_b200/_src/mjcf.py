@@ -301,6 +301,39 @@ def contact_slot_size(dataspec: int) -> int:
   return sum(n for i, (_, n) in enumerate(CONTACT_DATA) if dataspec >> i & 1)
 
 
+# the object attributes of the camprojection / insidesite / tendon sensors: (attribute, object type, name list) of the
+# sensor's object, then of its reference object (None: no reference)
+_EXTRA_SENSOR_ATTRS = {
+  "camprojection": (("site", C.OBJ_SITE, "site"), ("camera", C.OBJ_CAMERA, "camera")),
+  "insidesite": (("objname", None, None), ("site", C.OBJ_SITE, "site")),
+  **{t: (("tendon", C.OBJ_TENDON, "tendon"), None) for t in ("tendonlimitpos", "tendonlimitvel", "tendonlimitfrc", "tendonactfrc")},
+}
+
+
+def _extra_sensor_objects(e, names, objtypes, what):
+  """((objtype, objid), (reftype, refid)) of a camprojection / insidesite / tendon sensor element; ValueError naming the
+  sensor for a missing attribute, an unknown name or an insidesite objtype other than body, xbody, geom, site or camera."""
+  out = []
+  for spec in _EXTRA_SENSOR_ATTRS[e.tag]:
+    if spec is None:
+      out.append((C.OBJ_UNKNOWN, -1))
+      continue
+    attr, typ, lst = spec
+    if typ is None:  # insidesite's object: objtype= and objname=
+      if e.get("objtype") is None:
+        raise ValueError(f"{what}: missing attribute objtype")
+      if e.get("objtype") not in objtypes:
+        raise ValueError(f"{what}: objtype '{e.get('objtype')}' is not one of {', '.join(objtypes)}")
+      typ, lst = objtypes[e.get("objtype")]
+    if e.get(attr) is None:
+      raise ValueError(f"{what}: missing attribute {attr}")
+    lst_names = getattr(names, lst)
+    if e.get(attr) not in lst_names:
+      raise ValueError(f"{what}: unknown {lst} '{e.get(attr)}' in {attr}")
+    out.append((typ, lst_names.index(e.get(attr))))
+  return out
+
+
 def contact_intprm(data, reduce, num, what):
   """(dataspec, reduce, num) of a <contact> sensor's data / reduce / num attributes; ValueError naming `what` for an unknown or
   out-of-order data keyword, an unknown reduce value or num < 1."""
@@ -1634,6 +1667,13 @@ def compile_xml(root):
     "e_potential": (S.SENS_E_POTENTIAL, None, 1, 0, 1), "e_kinetic": (S.SENS_E_KINETIC, None, 1, 0, 1),
     # contacts matched against up to two sides; dim is num x the slot size of its data keywords (below)
     "contact": (S.SENS_CONTACT, "contact", 0, 0, 3),
+    # a site's pixel in a camera's image, an object's point inside a site's volume (0 / 1).  `<magnetometer>` stays in
+    # sensor_unsupported: put_model runs magnetometers of models that carry them in their arrays (sensor_type MAGNETOMETER on a site).
+    "camprojection": (S.SENS_CAMPROJECTION, "extra", 2, 0, 1),
+    "insidesite": (S.SENS_INSIDESITE, "extra", 1, 0, 1),
+    # a tendon's limit row (distance - margin, velocity, force; 0 without an active row) and the force of the actuators on it
+    "tendonlimitpos": (S.SENS_TENDONLIMITPOS, "extra", 1, 0, 1), "tendonlimitvel": (S.SENS_TENDONLIMITVEL, "extra", 1, 0, 2),
+    "tendonlimitfrc": (S.SENS_TENDONLIMITFRC, "extra", 1, 0, 3), "tendonactfrc": (S.SENS_TENDONACTFRC, "extra", 1, 0, 3),
   }
   objkind = {"tendon": (C.OBJ_TENDON, "tendon"), "joint": (C.OBJ_JOINT, "joint"), "actuator": (C.OBJ_ACTUATOR, "actuator"), "site": (C.OBJ_SITE, "site"), "body": (C.OBJ_BODY, "body")}
   objtypes = {"body": (C.OBJ_BODY, "body"), "xbody": (C.OBJ_XBODY, "body"), "geom": (C.OBJ_GEOM, "geom"), "site": (C.OBJ_SITE, "site"), "camera": (C.OBJ_CAMERA, "camera")}
@@ -1681,6 +1721,8 @@ def compile_xml(root):
       (otype, oid), (rtype, rid) = sides
       intprm = contact_intprm(e.get("data", "found"), e.get("reduce", "none"), e.get("num", "1"), f"contact sensor '{sname}'")
       dim = intprm[2] * contact_slot_size(intprm[0])
+    elif kind == "extra":
+      (otype, oid), (rtype, rid) = _extra_sensor_objects(e, m.names, objtypes, f"{e.tag} sensor '{e.get('name', f'sensor{len(sens)}')}'")
     elif kind == "obj":
       otype, lst = objtypes[e.get("objtype")]
       oid = getattr(m.names, lst).index(e.get("objname"))

@@ -107,6 +107,7 @@ int mjb_model_set_int(mjbModel* m, const char* name, int v) {
     return 0;
   }
   if (!strcmp(name, "nsensorcontact")) { m->scon.nsensorcontact = v; return 0; }
+  if (!strcmp(name, "sensor_extra")) { m->dev.sensor_extra = v; return 0; }
 #define X(n) if (!strcmp(name, #n)) { m->en.n = v; return 0; }
   MJB_ENERGY_INTS(X)
 #undef X
@@ -156,14 +157,17 @@ int mjb_model_set_array_batched(mjbModel* m, const char* name, const void* p, in
     m->setc.meaninertia = (float*)p;
     return 0;
   }
+  if (!strcmp(name, "cam_resolution")) { if (nbatch != 1) return fail("integer Model tables are shared by all worlds (not batched): cam_resolution"); m->dev.cam_resolution = (const int*)p; return 0; }
 #define X(n) if (!strcmp(name, #n)) { m->dev.n = (const float*)p; m->dev.nb_##n = nbatch; m->dev.bs_##n = batch_stride; goto done; }
   MJB_MODEL_FARRS(X)
+  MJB_MODEL_SENSOR_FARRS(X)
 #undef X
   return fail(std::string("unknown model array field: ") + name);
 done:
   m->dev.batched = 0;
 #define X(n) if (m->dev.nb_##n > 1) m->dev.batched = 1;
   MJB_MODEL_FARRS(X)
+  MJB_MODEL_SENSOR_FARRS(X)
 #undef X
   return 0;
 }
@@ -175,6 +179,8 @@ int mjb_model_finalize(mjbModel* m) {
 #define X(n) if (!m->dev.n) return fail(std::string("model array not set: ") + #n);
   MJB_MODEL_IARRS(X)
   MJB_MODEL_FARRS(X)
+  MJB_MODEL_SENSOR_FARRS(X)
+  X(cam_resolution)
 #undef X
 #define X(n) if (!m->fluid.n) return fail(std::string("model array not set: ") + #n);
   MJB_FLUID_IARRS(X)

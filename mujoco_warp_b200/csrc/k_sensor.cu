@@ -2,13 +2,16 @@
 //
 // Replaces (reference, /root/reference/mujoco_warp/_src/): sensor.py:810 sensor_pos, :1432 sensor_vel, :2512 sensor_acc for the sensor
 // types this build carries (joint / actuator / ball readings, gyro, velocimeter, accelerometer, subtree com / linvel / angmom, frame
-// position and axes, clock), with their prerequisites smooth.py:3500-3612 subtree_vel (subtree linear velocity and angular momentum) and
+// position and axes, clock; with EXTRA also magnetometer, camprojection, insidesite, tendon limit pos / vel / frc and tendonactfrc,
+// mjb_sensor_extra.cuh), with their prerequisites smooth.py:3500-3612 subtree_vel (subtree linear velocity and angular momentum) and
 // smooth.py:1743 rne_postconstraint (cfrc_ext from applied wrenches, body-to-body connect / weld equalities and contacts; cacc including
 // qacc; cfrc_int accumulated up the tree).  Every input a position- or velocity-stage sensor reads is final once its stage has run, so one launch after
-// the solver evaluates all three stages (the stage mask lets sensor_pos / sensor_vel / sensor_acc be called on their own).
+// the solver evaluates all three stages (the stage mask lets sensor_pos / sensor_vel / sensor_acc be called on their own).  EXTRA is
+// chosen per model (ModelDev.sensor_extra), so a model without those sensor types runs the same code as before they existed.
 #include "mjb_launch.cuh"
 #include "mjb_math.cuh"
 #include "mjb_ray.cuh"
+#include "mjb_sensor_extra.cuh"
 #include "mjb_types.cuh"
 
 namespace {
@@ -49,7 +52,7 @@ __device__ __forceinline__ int obj_body(const ModelDev& m, int objtype, int id) 
   }
 }
 
-template <bool BAT>
+template <bool BAT, bool EXTRA>
 __global__ void __launch_bounds__(32)
 k_sensor(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d, int stages) {
   extern __shared__ float smem[];  // nbody x (linvel 3 | angmom 3 | bodyvel lin 3) or nbody x (cfrc_ext 6 | cacc / cfrc_int 6)
@@ -344,7 +347,31 @@ k_sensor(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d,
         v[0] = r.x; v[1] = r.y; v[2] = r.z; break; }
       case SENS_ACTUATORFRC: v[0] = d.actuator_force[wb * m.nu + id]; break;
       case SENS_JOINTACTFRC: v[0] = d.qfrc_actuator[wb * nv + m.jnt_dofadr[id]]; break;
-      default: continue;
+      default: {
+        if (!EXTRA) continue;
+        switch (t) {  // mjb_sensor_extra.cuh
+          case SENS_MAGNETOMETER: { const v3 r = sensor_magnetometer(d.site_xmat + (wb * m.nsite + id) * 9, ld3(m.magnetic)); v[0] = r.x; v[1] = r.y; v[2] = r.z; break; }
+          case SENS_CAMPROJECTION:
+            sensor_camprojection(ld3(d.site_xpos + (wb * m.nsite + id) * 3), ld3(d.cam_xpos + (wb * m.ncam + rid) * 3), d.cam_xmat + (wb * m.ncam + rid) * 9, m.cam_fovy[rid],
+                                 m.cam_intrinsic + 4 * rid, m.cam_sensorsize + 2 * rid, m.cam_resolution + 2 * rid, v);
+            break;
+          case SENS_INSIDESITE: {
+            const int ot = m.sensor_objtype[s];
+            const v3 p = sensor_inside_point(ot, id, obj_pos(d, m, wb, ot, id), d.subtree_com + (wb * nb + id) * 3, ot == OBJ_BODY ? m.body_mass[id] : 0.f,
+                                             ot == OBJ_BODY ? m.body_subtreemass[id] : 0.f);
+            v[0] = contact_inside_site(ld3(d.site_xpos + (wb * m.nsite + rid) * 3), d.site_xmat + (wb * m.nsite + rid) * 9, ld3(m.site_size + 3 * rid), m.site_type[rid], p) ? 1.f : 0.f;
+            break; }
+          case SENS_TENDONLIMITPOS: case SENS_TENDONLIMITVEL: case SENS_TENDONLIMITFRC: {  // sensor.py:228, :1028, :1640: the tendon's limit row, else 0
+            const int e0 = d.ne[w] + d.nf[w], e1 = min(e0 + d.nl[w], d.njmax);
+            for (int e = e0; e < e1; e++)
+              if (d.efc_id[wb * d.njmax + e] == id && d.efc_type[wb * d.njmax + e] == CNSTR_LIMIT_TENDON)
+                v[0] = t == SENS_TENDONLIMITPOS ? d.efc_pos[wb * d.njmax + e] - d.efc_margin[wb * d.njmax + e]
+                                                : (t == SENS_TENDONLIMITVEL ? d.efc_vel[wb * d.njmax + e] : d.efc_force[wb * d.njmax + e]);
+            break; }
+          case SENS_TENDONACTFRC: v[0] = sensor_tendon_actfrc(m.nu, m.actuator_trntype, m.actuator_trnid, d.actuator_force + wb * m.nu, id); break;
+          default: continue;
+        }
+      }
     }
     // sensor.py:56-113: cutoff clamps REAL data to [-c, c] and POSITIVE data from above
     const float cutoff = m.sensor_cutoff[s];
@@ -361,7 +388,10 @@ k_sensor(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d,
 
 cudaError_t launch_sensor(const ModelDev& m, const DataDev& d, int stages, cudaStream_t s, const SensorCollisionDev& c) {
   if (m.nsensor == 0) return cudaSuccess;
-  const cudaError_t e = launch(m.batched ? k_sensor<true> : k_sensor<false>, d.wn, 32, (size_t)12 * m.nbody * sizeof(float), s, m, d, stages);
+  // models with a magnetometer / camprojection / insidesite / tendon limit / tendonactfrc sensor run the EXTRA build; the others the
+  // plain one, whose switch does not know those types
+  const cudaError_t e = launch(m.sensor_extra ? (m.batched ? k_sensor<true, true> : k_sensor<false, true>) : (m.batched ? k_sensor<true, false> : k_sensor<false, false>),
+                               d.wn, 32, (size_t)12 * m.nbody * sizeof(float), s, m, d, stages);
   // k_sensor skips the collision sensors: their slots are k_sensor_collision's
   if (e != cudaSuccess || !(stages & STAGE_POS) || c.nsensorcollision == 0 || (m.disableflags & DSBL_SENSOR)) return e;
   return launch_sensor_collision(m, d, c, s);

@@ -40,6 +40,8 @@
   X(wrap_prm) X(ten_J0) X(tendon_range) X(tendon_margin) X(tendon_stiffness) X(tendon_damping) X(tendon_frictionloss) X(tendon_lengthspring) \
   X(tendon_length0) X(tendon_invweight0) X(tendon_solref_lim) X(tendon_solimp_lim) X(tendon_solref_fri) X(tendon_solimp_fri) X(tendon_actfrcrange) \
   X(geom_rgba) X(mat_rgba) X(actuator_acc0) X(actuator_lengthrange)
+// opt.magnetic (nb, 3), cam_fovy (nb, ncam), cam_intrinsic (nb, ncam, 4), cam_sensorsize (ncam, 2): batched like MJB_MODEL_FARRS
+#define MJB_MODEL_SENSOR_FARRS(X) X(magnetic) X(cam_fovy) X(cam_intrinsic) X(cam_sensorsize)
 
 struct ModelDev {
 #define X(n) int n;
@@ -60,6 +62,13 @@ struct ModelDev {
 #define X(n) int nb_##n, bs_##n;
   MJB_MODEL_FARRS(X)
 #undef X
+  // fields only the magnetometer / camprojection / insidesite / tendon sensors read (k_sensor's EXTRA build): appended after every other
+  // field, so that the parameter offsets of every other kernel stay where they were
+  int sensor_extra;                                  // the model has a sensor of one of those types (selects k_sensor<BAT, true>)
+  const int* __restrict__ cam_resolution;            // (ncam, 2)
+#define X(n) const float* __restrict__ n; int nb_##n, bs_##n;
+  MJB_MODEL_SENSOR_FARRS(X)
+#undef X
 };
 
 #ifdef __CUDACC__
@@ -69,6 +78,7 @@ __device__ __forceinline__ ModelDev world_model(const ModelDev& m, int w, int nw
   ModelDev r = m;
 #define X(n) if (m.nb_##n > 1) r.n = m.n + (size_t)(m.nb_##n == nworld ? w : w % m.nb_##n) * (size_t)m.bs_##n;
   MJB_MODEL_FARRS(X)
+  MJB_MODEL_SENSOR_FARRS(X)
 #undef X
   return r;
 }
@@ -237,9 +247,10 @@ enum { EQ_CONNECT = 0, EQ_WELD = 1, EQ_JOINT = 2, EQ_TENDON = 3 };
 enum { TRN_JOINT = 0, TRN_TENDON = 3 };
 enum { OBJ_BODY = 1, OBJ_XBODY = 2, OBJ_GEOM = 5, OBJ_SITE = 6, OBJ_CAMERA = 7 };
 // mjtSensor values of the sensor types carried here (MuJoCo order, as in _src/constants.py)
-enum { SENS_TOUCH = 0, SENS_ACCELEROMETER = 1, SENS_VELOCIMETER = 2, SENS_GYRO = 3, SENS_FORCE = 4, SENS_TORQUE = 5, SENS_JOINTPOS = 9, SENS_JOINTVEL = 10, SENS_TENDONPOS = 11, SENS_TENDONVEL = 12, SENS_ACTUATORPOS = 13, SENS_ACTUATORVEL = 14,
-       SENS_ACTUATORFRC = 15, SENS_JOINTACTFRC = 16, SENS_BALLQUAT = 18, SENS_BALLANGVEL = 19, SENS_JOINTLIMITPOS = 20, SENS_JOINTLIMITVEL = 21, SENS_JOINTLIMITFRC = 22, SENS_FRAMEPOS = 26, SENS_FRAMEQUAT = 27, SENS_FRAMEXAXIS = 28,
-       SENS_FRAMEYAXIS = 29, SENS_FRAMEZAXIS = 30, SENS_FRAMELINVEL = 31, SENS_FRAMEANGVEL = 32, SENS_FRAMELINACC = 33, SENS_FRAMEANGACC = 34, SENS_SUBTREECOM = 35, SENS_SUBTREELINVEL = 36, SENS_SUBTREEANGMOM = 37, SENS_GEOMDIST = 39, SENS_GEOMNORMAL = 40,
+enum { SENS_TOUCH = 0, SENS_ACCELEROMETER = 1, SENS_VELOCIMETER = 2, SENS_GYRO = 3, SENS_FORCE = 4, SENS_TORQUE = 5, SENS_MAGNETOMETER = 6, SENS_CAMPROJECTION = 8, SENS_JOINTPOS = 9, SENS_JOINTVEL = 10, SENS_TENDONPOS = 11, SENS_TENDONVEL = 12, SENS_ACTUATORPOS = 13, SENS_ACTUATORVEL = 14,
+       SENS_ACTUATORFRC = 15, SENS_JOINTACTFRC = 16, SENS_TENDONACTFRC = 17, SENS_BALLQUAT = 18, SENS_BALLANGVEL = 19, SENS_JOINTLIMITPOS = 20, SENS_JOINTLIMITVEL = 21, SENS_JOINTLIMITFRC = 22, SENS_TENDONLIMITPOS = 23,
+       SENS_TENDONLIMITVEL = 24, SENS_TENDONLIMITFRC = 25, SENS_FRAMEPOS = 26, SENS_FRAMEQUAT = 27, SENS_FRAMEXAXIS = 28,
+       SENS_FRAMEYAXIS = 29, SENS_FRAMEZAXIS = 30, SENS_FRAMELINVEL = 31, SENS_FRAMEANGVEL = 32, SENS_FRAMELINACC = 33, SENS_FRAMEANGACC = 34, SENS_SUBTREECOM = 35, SENS_SUBTREELINVEL = 36, SENS_SUBTREEANGMOM = 37, SENS_INSIDESITE = 38, SENS_GEOMDIST = 39, SENS_GEOMNORMAL = 40,
        SENS_GEOMFROMTO = 41, SENS_E_POTENTIAL = 43, SENS_E_KINETIC = 44, SENS_CLOCK = 45 };
 enum { CNSTR_EQUALITY = 0, CNSTR_FRICTION_DOF = 1, CNSTR_FRICTION_TENDON = 2, CNSTR_LIMIT_JOINT = 3, CNSTR_LIMIT_TENDON = 4, CNSTR_CONTACT_FRICTIONLESS = 5, CNSTR_CONTACT_PYRAMIDAL = 6, CNSTR_CONTACT_ELLIPTIC = 7 };
 enum { ST_SATISFIED = 0, ST_QUADRATIC = 1, ST_LINEARNEG = 2, ST_LINEARPOS = 3, ST_CONE = 4 };
