@@ -32,6 +32,12 @@
  *   mjb_init_ctrl_history /    <- _src/history.py:796, :881  init_ctrl_history(m, d, ctrlid, times, values) /
  *     mjb_init_sensor_history       init_sensor_history(m, d, sensorid, times, values, phase)
  *   mjb_contact_force          <- _src/support.py:445  contact_force(m, d, contact_ids, to_world_frame, force)
+ *   mjb_rne_postconstraint     <- _src/smooth.py:1744  rne_postconstraint(m, d)
+ *   mjb_subtree_vel            <- _src/smooth.py:3614  subtree_vel(m, d)
+ *   mjb_tendon                 <- _src/smooth.py:4197  tendon(m, d) (fixed tendons: no wrap outputs)
+ *   mjb_jac                    <- _src/support.py:583  jac(m, d, jacp, jacr, point, body)
+ *   mjb_xfrc_accumulate        <- _src/support.py:314  xfrc_accumulate(m, d, qfrc)
+ *   mjb_deriv_smooth_vel       <- _src/derivative.py:1117  deriv_smooth_vel(m, d, out)
  *   mjb_rays                   <- _src/ray.py:1219 rays(m, d, pnt, vec, geomgroup, flg_static, bodyexclude, dist, geomid, normal) without a
  *                                 render context (every geom tested, no BVH; no height fields)
  *   mjb_refit_bvh              <- _src/bvh.py:39 refit_bvh(m, d, rc): world-space bounds of the rendered geoms (no BVH is built;
@@ -117,6 +123,23 @@ int mjb_mul_m(const mjbModel* m, mjbData* d, float* res, const float* vec, void*
 int mjb_sensor_pos(const mjbModel* m, mjbData* d, void* stream);
 int mjb_sensor_vel(const mjbModel* m, mjbData* d, void* stream);
 int mjb_sensor_acc(const mjbModel* m, mjbData* d, void* stream);
+/* Stages that read a finished forward pass, one kernel launch each over every world (see the exceptions below), whatever the model's sensors or DSBL_SENSOR say:
+ * smooth.py:1744 rne_postconstraint (Data.cacc, cfrc_int, cfrc_ext; contact and equality wrenches summed in pool / row order),
+ * smooth.py:3614 subtree_vel (Data.subtree_linvel, subtree_angmom), smooth.py:4197 tendon (Data.ten_length, ten_J of the fixed tendons; no
+ * launch without tendons). */
+int mjb_rne_postconstraint(const mjbModel* m, mjbData* d, void* stream);
+int mjb_subtree_vel(const mjbModel* m, mjbData* d, void* stream);
+int mjb_tendon(const mjbModel* m, mjbData* d, void* stream);
+/* support.py:583 jac: jacp / jacr (nworld, 3, nv) fp32 device (either may be NULL) = the translational / rotational Jacobian of point
+ * (nworld, 3) fp32 on body (nworld) int32; columns of dofs that do not move the body are 0; a body id outside [0, nbody) gives NaN rows.
+ * jac and xfrc_accumulate launch nothing for a model without dofs */
+int mjb_jac(const mjbModel* m, mjbData* d, float* jacp, float* jacr, const float* point, const int* body, void* stream);
+/* support.py:314 xfrc_accumulate: qfrc (nworld, nv) fp32 device += J^T Data.xfrc_applied, bodies summed in index order */
+int mjb_xfrc_accumulate(const mjbModel* m, mjbData* d, float* qfrc, void* stream);
+/* derivative.py:1117 deriv_smooth_vel: out (nworld, nC) fp32 device = M - dt qDeriv in Data.M's layout (M_rowadr / M_colind); qDeriv: affine
+ * actuators (unless DSBL_ACTUATION), dof and tendon damping (unless DSBL_DAMPER), fluid forces (an ellipsoid's derivative symmetrized for the
+ * implicitfast integrator only, as the reference does) */
+int mjb_deriv_smooth_vel(const mjbModel* m, mjbData* d, float* out, void* stream);
 /* sensor.py:2934 energy_pos / :3004 energy_vel: Data.energy[:, 0] = potential energy (gravity unless DSBL_GRAVITY; joint and fixed-tendon
  * springs unless DSBL_SPRING) at the last position stage; Data.energy[:, 1] = 1/2 qvel . M qvel with the M of the last crb.  Whatever
  * ENBL_ENERGY says; one kernel launch each.  Data.energy is bound by name ("energy", (nworld, 2) fp32).  forward / step / step1 compute

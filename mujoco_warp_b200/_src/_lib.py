@@ -15,7 +15,7 @@ _PKG = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 _CSRC = os.path.join(_PKG, "csrc")
 LIB_PATH = os.environ.get("MJB_LIB", os.path.join(_PKG, "libmjb200.so"))  # MJB_LIB: A/B-test an alternative build
 HEADER_PATH = os.path.join(os.path.dirname(_PKG), "include", "mjb200.h")
-SOURCES = ["capi.cu", "k_position.cu", "k_collision.cu", "k_collision_mesh.cu", "k_collision_mesh_large.cu", "k_constraint.cu", "k_velocity.cu", "k_solver.cu", "k_integrate.cu", "k_implicit.cu", "k_support.cu", "k_sensor.cu", "k_sensor_collision.cu", "k_sensor_collision_large.cu", "k_sensor_contact.cu", "k_ray.cu", "k_inverse.cu", "k_set_const.cu", "k_energy.cu", "k_history.cu", "k_render.cu"]
+SOURCES = ["capi.cu", "k_position.cu", "k_collision.cu", "k_collision_mesh.cu", "k_collision_mesh_large.cu", "k_constraint.cu", "k_velocity.cu", "k_solver.cu", "k_integrate.cu", "k_implicit.cu", "k_support.cu", "k_sensor.cu", "k_sensor_collision.cu", "k_sensor_collision_large.cu", "k_sensor_contact.cu", "k_ray.cu", "k_inverse.cu", "k_set_const.cu", "k_energy.cu", "k_history.cu", "k_render.cu", "k_body_stages.cu"]
 NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a", "--extended-lambda", "-Xcompiler", "-fPIC", "-shared"]
 
 _lib = None
@@ -125,6 +125,11 @@ def lib():
   for f, args in (("mjb_read_ctrl", [vp, ci, vp]), ("mjb_read_sensor", [vp, ci, vp]), ("mjb_init_ctrl_history", [vp, vp]), ("mjb_init_sensor_history", [vp, vp, vp])):
     getattr(L, f).argtypes = [vp, vp, ci] + args + [vp]
     getattr(L, f).restype = ci
+  L.mjb_jac.argtypes = [vp, vp, vp, vp, vp, vp, vp]
+  L.mjb_jac.restype = ci
+  for f in ("mjb_xfrc_accumulate", "mjb_deriv_smooth_vel"):
+    getattr(L, f).argtypes = [vp, vp, vp, vp]
+    getattr(L, f).restype = ci
   L.mjb_step_profile.argtypes = [vp, vp, vp, ctypes.POINTER(ctypes.c_float)]
   L.mjb_last_launch_count.restype = ci
   L.mjb_collision_kernel.argtypes = [vp]
@@ -137,7 +142,7 @@ STAGE_FUNCS = [
   "mjb_step", "mjb_forward", "mjb_inverse", "mjb_fwd_position", "mjb_kinematics", "mjb_com_pos", "mjb_camlight", "mjb_crb", "mjb_transmission",
   "mjb_collision", "mjb_make_constraint", "mjb_fwd_velocity", "mjb_fwd_actuation", "mjb_fwd_acceleration", "mjb_factor_m",
   "mjb_solve", "mjb_euler", "mjb_implicit", "mjb_com_vel", "mjb_passive", "mjb_rne", "mjb_rungekutta4", "mjb_sensor_pos", "mjb_sensor_vel", "mjb_sensor_acc",
-  "mjb_energy_pos", "mjb_energy_vel",
+  "mjb_energy_pos", "mjb_energy_vel", "mjb_rne_postconstraint", "mjb_subtree_vel", "mjb_tendon",
 ]
 
 

@@ -192,6 +192,66 @@ def contact_force(m: Model, d: Data, contact_ids: torch.Tensor, to_world_frame: 
   _lib.check(_lib.lib().mjb_contact_force(m._handle, d._handle, contact_ids.data_ptr(), n, int(bool(to_world_frame)), force.data_ptr(), stream))
 
 
+def rne_postconstraint(m: Model, d: Data):
+  """Per-body accelerations d.cacc, internal wrenches d.cfrc_int and external wrenches d.cfrc_ext (applied, connect / weld equality and
+  contact) after the constraint solve (reference smooth.py:1744).  Reads the finished forward pass; runs whatever the model's sensors or
+  DisableBit.SENSOR say.  Equality and contact wrenches are summed in row and contact-pool order, so the result is bit-reproducible."""
+  _call("mjb_rne_postconstraint", m, d)
+
+
+def subtree_vel(m: Model, d: Data):
+  """Subtree linear velocity d.subtree_linvel and angular momentum d.subtree_angmom of every body (reference smooth.py:3614).  Reads the
+  last position and velocity stages; runs whatever the model's sensors or DisableBit.SENSOR say."""
+  _call("mjb_subtree_vel", m, d)
+
+
+def tendon(m: Model, d: Data):
+  """Fixed-tendon lengths d.ten_length and Jacobians d.ten_J at the current qpos (reference smooth.py:4197); only fixed tendons exist here,
+  so there are no wrap outputs.  Launches nothing for a model without tendons."""
+  _call("mjb_tendon", m, d)
+
+
+def _check_f32(name: str, t, shape):
+  if not isinstance(t, torch.Tensor) or t.dtype != torch.float32 or not t.is_cuda or not t.is_contiguous() or tuple(t.shape) != tuple(shape):
+    raise ValueError(f"{name}: expected a contiguous CUDA float32 tensor of shape {tuple(shape)}")
+
+
+def jac(m: Model, d: Data, jacp: torch.Tensor | None, jacr: torch.Tensor | None, point: torch.Tensor, body: torch.Tensor):
+  """Translational (jacp) and rotational (jacr) Jacobian of a world-frame point on a body, one per world (reference support.py:583).
+
+  point: (nworld, 3) float32; body: (nworld,) int32 body ids; jacp / jacr: (nworld, 3, nv) float32 outputs, either may be None.  Every
+  entry is written: columns of dofs that do not move the body are 0.  A body id outside [0, nbody) cannot be checked without a
+  synchronisation: that world's rows are written as NaN instead.  A model without dofs launches nothing."""
+  nw = d.nworld
+  _check_f32("point", point, (nw, 3))
+  if not isinstance(body, torch.Tensor) or body.dtype != torch.int32 or not body.is_cuda or not body.is_contiguous() or tuple(body.shape) != (nw,):
+    raise ValueError(f"body: expected a contiguous CUDA int32 tensor of shape ({nw},)")
+  for name, t in (("jacp", jacp), ("jacr", jacr)):
+    if t is not None:
+      _check_f32(name, t, (nw, 3, m.nv))
+  stream = torch.cuda.current_stream().cuda_stream
+  ptr = lambda t: t.data_ptr() if t is not None else None
+  _lib.check(_lib.lib().mjb_jac(m._handle, d._handle, ptr(jacp), ptr(jacr), point.data_ptr(), body.data_ptr(), stream))
+
+
+def xfrc_accumulate(m: Model, d: Data, qfrc: torch.Tensor):
+  """Adds d.xfrc_applied, mapped to joint space through each body's Jacobian at its centre of mass, into qfrc (nworld, nv) float32
+  (reference support.py:314).  Bodies are summed in index order, so the result is bit-reproducible."""
+  _check_f32("qfrc", qfrc, (d.nworld, m.nv))
+  stream = torch.cuda.current_stream().cuda_stream
+  _lib.check(_lib.lib().mjb_xfrc_accumulate(m._handle, d._handle, qfrc.data_ptr(), stream))
+
+
+def deriv_smooth_vel(m: Model, d: Data, out: torch.Tensor):
+  """out (nworld, nC) float32 = M - dt qDeriv in the layout of d.M (M_rowadr / M_colind), for any integrator (reference
+  derivative.py:1117).  qDeriv holds the derivatives of the smooth forces with respect to qvel: affine actuator gain / bias (unless
+  DisableBit.ACTUATION), dof and tendon damping (unless DisableBit.DAMPER), and the fluid forces of a model that has them.  As in the
+  reference, an ellipsoid's fluid derivative is symmetrized when the model's integrator is implicitfast and used as it stands otherwise."""
+  _check_f32("out", out, (d.nworld, m.nC))
+  stream = torch.cuda.current_stream().cuda_stream
+  _lib.check(_lib.lib().mjb_deriv_smooth_vel(m._handle, d._handle, out.data_ptr(), stream))
+
+
 _STATE_ORDER = ("TIME", "QPOS", "QVEL", "ACT", "HISTORY", "WARMSTART", "CTRL", "QFRC_APPLIED", "XFRC_APPLIED", "EQ_ACTIVE", "MOCAP_POS", "MOCAP_QUAT", "USERDATA")
 
 

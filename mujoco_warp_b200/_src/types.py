@@ -109,6 +109,18 @@ class OverflowType(enum.IntFlag):
   LS_ITERATIONS = 1 << 10
 
 
+class ObjType(enum.IntEnum):
+  """Object types (MuJoCo mjtObj values; reference types.py:651).  XBODY addresses a body's regular frame instead of its inertial one."""
+
+  UNKNOWN = 0
+  BODY = 1
+  XBODY = 2
+  GEOM = 5
+  FLEX = 9
+  SITE = 6
+  CAMERA = 7
+
+
 class BroadphaseType(enum.IntEnum):
   NXN = 0
   SAP_TILE = 1

@@ -397,6 +397,31 @@ int mjb_contact_force(const mjbModel* m, mjbData* d, const int* contact_ids, int
   MJB_LAUNCH(launch_contact_force(m->dev, d->dev, contact_ids, n, to_world_frame, force, s));
   return 0;
 }
+// smooth.py:1744 rne_postconstraint, :3614 subtree_vel, :4197 tendon; support.py:583 jac, :314 xfrc_accumulate; derivative.py:1117
+// deriv_smooth_vel: one launch each over every world (none for tendon without tendons, nor for jac / xfrc_accumulate without dofs),
+// whatever the model's sensors or DSBL_SENSOR say
+int mjb_rne_postconstraint(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_rne_postconstraint(m->dev, d->dev, s)); return 0; }
+int mjb_subtree_vel(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_subtree_vel(m->dev, d->dev, s)); return 0; }
+int mjb_tendon(const mjbModel* m, mjbData* d, void* stream) { MJB_ENTER(); MJB_LAUNCH(launch_tendon(m->dev, d->dev, s)); return 0; }
+int mjb_jac(const mjbModel* m, mjbData* d, float* jacp, float* jacr, const float* point, const int* body, void* stream) {
+  MJB_ENTER();
+  if (!point || !body) return fail("mjb_jac: null point / body array");
+  MJB_LAUNCH(launch_jac(m->dev, d->dev, jacp, jacr, point, body, s));
+  return 0;
+}
+int mjb_xfrc_accumulate(const mjbModel* m, mjbData* d, float* qfrc, void* stream) {
+  MJB_ENTER();
+  if (!qfrc) return fail("mjb_xfrc_accumulate: null qfrc");
+  MJB_LAUNCH(launch_xfrc_accumulate(m->dev, d->dev, qfrc, s));
+  return 0;
+}
+int mjb_deriv_smooth_vel(const mjbModel* m, mjbData* d, float* out, void* stream) {
+  MJB_ENTER();
+  if (!out) return fail("mjb_deriv_smooth_vel: null out");
+  if (smem_deriv_smooth_vel(m->dev) > kMaxSmem) return fail("mjb_deriv_smooth_vel: the largest tree's block exceeds one block's shared memory");
+  MJB_LAUNCH(launch_deriv_smooth_vel(m->dev, d->dev, out, s, fluid(m, d)));
+  return 0;
+}
 int mjb_rays(const mjbModel* m, mjbData* d, const float* pnt, const float* vec, int nray, int pnt_nbatch, const int* geomgroup, int flg_static,
              const int* bodyexclude, float* dist, int* geomid, float* normal, void* stream) {
   MJB_ENTER();

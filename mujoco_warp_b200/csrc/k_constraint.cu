@@ -83,13 +83,7 @@ __device__ void efc_row(const ModelDev& m, const DataDev& d, int w, int efcid, f
 // are read from Data as the previous velocity stage left them (the reference builds constraints before fwd_velocity too).
 __device__ __forceinline__ void jac_cols(const ModelDev& m, const DataDev& d, size_t wb, const float* cdof, const float* scom, v3 point, int b,
                                          int dof, v3* jp, v3* jr, v3* dp, v3* dr) {
-  *jp = *jr = *dp = *dr = mk3(0.f, 0.f, 0.f);
-  if (!m.body_isdofancestor[b * m.nv + dof]) return;
-  const v3 off = point - ld3(scom + 3 * m.body_rootid[b]);
-  const float* cd = cdof + 6 * dof;
-  const v3 cang = ld3(cd), clin = ld3(cd + 3);
-  *jp = clin + cross(cang, off);
-  *jr = cang;
+#include "k_body_jac.cuh"
   const float* cv = d.cvel + (wb * m.nbody + b) * 6;
   const v3 pvel = ld3(cv + 3) - cross(off, ld3(cv));
   float cdd[6];

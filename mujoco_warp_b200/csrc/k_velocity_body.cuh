@@ -352,19 +352,7 @@
       if (team_any<LPW>(any_xfrc, g)) {
 #pragma unroll 1
         for (int dd = sub; dd < nv; dd += LPW) {
-          const float* cd = cdof + 6 * dd;
-          const int db = m.dof_bodyid[dd];
-          float acc = 0.f;
-          for (int b = db; b < nb; b++) {
-            const float* ft = d.xfrc_applied + (wb * nb + b) * 6;
-            if (ft[0] == 0.f && ft[1] == 0.f && ft[2] == 0.f && ft[3] == 0.f && ft[4] == 0.f && ft[5] == 0.f) continue;
-            int p = b;
-            while (p != 0 && p != db) p = m.body_parentid[p];
-            if (p == 0) continue;
-            const v3 off = ld3(d.xipos + (wb * nb + b) * 3) - ld3(d.subtree_com + (wb * nb + m.body_rootid[b]) * 3);
-            const v3 cr = cross(ld3(cd), off);
-            acc += cd[3] * ft[0] + cd[4] * ft[1] + cd[5] * ft[2] + cd[0] * ft[3] + cd[1] * ft[4] + cd[2] * ft[5] + dot(cr, ld3(ft));
-          }
+#include "k_body_xfrc.cuh"
           q_smooth[dd] += acc;
         }
       }

@@ -198,7 +198,8 @@ static __device__ __forceinline__ void fluid_box_B(const ModelDev& m, const Flui
 }
 
 // derivative.py:588-852 _deriv_ellipsoid_fluid for one geom: B (6 x 6, row-major, rows and columns [angular; linear]) at the geom's
-// local velocity, symmetrized as for implicitfast.
+// local velocity, symmetrized as for implicitfast (SYM); without SYM as it stands, as derivative.py:800 leaves it for the other integrators.
+template <bool SYM = true>
 static __device__ void fluid_ellipsoid_B(const float* fl, v3 s, v3 ang_vel, v3 lin_vel, float density, float viscosity, float* B) {
   const float PI = 3.14159265358979323846f;
   float B00[9], B01[9], B10[9], B11[9];
@@ -276,6 +277,7 @@ static __device__ void fluid_ellipsoid_B(const float* fl, v3 s, v3 ang_vel, v3 l
   const float diag_val = dot(ang_vel, mom_sq) - viscosity * lin_visc_torq_coef;
   for (int r = 0; r < 3; r++)
     for (int q = 0; q < 3; q++) B00[3 * r + q] += fl_comp(ang_vel, r) * fl_comp(mom_sq, q) + (r == q ? diag_val : 0.f);
+  if constexpr (SYM) {
   // symmetrize (implicitfast) into B
   for (int r = 0; r < 3; r++)
     for (int q = 0; q < 3; q++) {
@@ -285,6 +287,15 @@ static __device__ void fluid_ellipsoid_B(const float* fl, v3 s, v3 ang_vel, v3 l
       B[6 * r + q + 3] = b01;
       B[6 * (q + 3) + r] = b01;
     }
+  } else {
+    for (int r = 0; r < 3; r++)
+      for (int q = 0; q < 3; q++) {
+        B[6 * r + q] = B00[3 * r + q];
+        B[6 * r + q + 3] = B01[3 * r + q];
+        B[6 * (r + 3) + q] = B10[3 * r + q];
+        B[6 * (r + 3) + q + 3] = B11[3 * r + q];
+      }
+  }
 }
 
 // The local Jacobian column of dof dd at a point with offset `off` from the subtree root's com, in the frame R: [R^T ang; R^T lin].

@@ -13,8 +13,9 @@
 // Writes the lower triangle of the block of tree dofs [start, start + n) of world wb (Mw: its M values) into A (row-major, leading
 // dimension ld; the upper triangle is zeroed); f: the model's fluid fields, read with FLUID only.  damper: add dt * dof_damping on the diagonal; implicitfast: subtract dt times the actuator and add dt times the tendon damping
 // derivatives on the entries of the M sparsity pattern, and with FLUID (a model with fluid forces) the fluid force derivatives.  The warp's
-// lanes share the work; ends with the warp converged.
-template <bool FLUID = false>
+// lanes share the work; ends with the warp converged.  SYM: the fluid B of an ellipsoid is symmetrized, as implicitfast does
+// (derivative.py:800); deriv_smooth_vel for the other integrators leaves it as it stands (the inertia-box B is diagonal either way).
+template <bool FLUID = false, bool SYM = true>
 __device__ __forceinline__ void tree_implicit_a(const ModelDev& m, const DataDev& d, size_t wb, const float* Mw, int start, int n, int ld, float dt,
                                                 bool implicitfast, bool damper, float* A, int lane, const FluidDev& f) {
   const int nv = m.nv;
@@ -121,7 +122,7 @@ __device__ __forceinline__ void tree_implicit_a(const ModelDev& m, const DataDev
           v3 l_lin = fl_mtv(R, lin + cross(ang, gpos - xip));
           if (has_wind) l_lin = l_lin - fl_mtv(R, wind);
           float B[36];
-          fluid_ellipsoid_B(fl, fluid_semiaxes(m.geom_type[g], m.geom_size + 3 * g), l_ang, l_lin, f.density, f.viscosity, B);
+          fluid_ellipsoid_B<SYM>(fl, fluid_semiaxes(m.geom_type[g], m.geom_size + 3 * g), l_ang, l_lin, f.density, f.viscosity, B);
 #pragma unroll 1
           for (int e = e0 + lane; e < e1; e += 32) {
             const int r = m.M_entry_row[e], col = m.M_colind[e];

@@ -342,6 +342,16 @@ cudaError_t launch_set_length_range(const ModelDev& m, int nw, int nworld, cudaS
 // energy (k_energy.cu): the ENERGY_* parts of d's world range
 cudaError_t launch_energy(const ModelDev& m, const DataDev& d, const EnergyDev& e, int parts, cudaStream_t s);
 size_t smem_integrate(const ModelDev& m);
+// the individually callable stages that read a finished forward pass (k_body_stages.cu), each over d's world range: cacc / cfrc_int /
+// cfrc_ext; subtree_linvel / subtree_angmom; the (nworld, 3, nv) Jacobians of point (nworld, 3) on body (nworld) into jacp / jacr (either
+// may be null); qfrc (nworld, nv) += J^T xfrc_applied; ten_length / ten_J (no launch without tendons); out (nworld, nC) = M - dt qDeriv
+cudaError_t launch_rne_postconstraint(const ModelDev& m, const DataDev& d, cudaStream_t s);
+cudaError_t launch_subtree_vel(const ModelDev& m, const DataDev& d, cudaStream_t s);
+cudaError_t launch_jac(const ModelDev& m, const DataDev& d, float* jacp, float* jacr, const float* point, const int* body, cudaStream_t s);
+cudaError_t launch_xfrc_accumulate(const ModelDev& m, const DataDev& d, float* qfrc, cudaStream_t s);
+cudaError_t launch_tendon(const ModelDev& m, const DataDev& d, cudaStream_t s);
+cudaError_t launch_deriv_smooth_vel(const ModelDev& m, const DataDev& d, float* out, cudaStream_t s, const FluidDev& f);
+size_t smem_deriv_smooth_vel(const ModelDev& m);
 // actuator and sensor delays (k_history.cu), each over d's world range: the delayed ctrl into h.ctrl_delayed; d.ctrl inserted at
 // d.time; the sensors of `stages` (1 pos, 2 vel, 4 acc) replaced by their delayed / held values, the fresh ones inserted
 cudaError_t launch_history_ctrl_read(const ModelDev& m, const DataDev& d, const HistoryDev& h, cudaStream_t s);
