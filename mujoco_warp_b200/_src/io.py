@@ -649,7 +649,7 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   m.ten_J0 = dev_f(tenJ0, batched=False)
   for n, k in _TENDON_FLOATS:
     setattr(m, n, dev_f(np.asarray(getattr(mjm, n)).reshape((nt, k) if k > 1 else (nt,)) if nt else np.zeros((0, k) if k > 1 else 0), name=n))
-  m.ntenfric = int((np.asarray(mjm.tendon_frictionloss) > 0).sum()) if nt else 0
+  t["dof_fricloss_adr"], m.ntenfric = _fricloss_tables(m.dof_frictionloss, m.tendon_frictionloss)
   m.jnt_limited = dev_i(np.asarray(mjm.jnt_limited).astype(np.int32))
   m.body_tree = tuple(dev_i(x) for x in t["body_tree"])
   for n in ("body_childadr", "body_childid", "level_adr", "level_body", "M_entry_row", "mulm_rowadr", "mulm_col", "mulm_madr", "tree_qLDadr",
@@ -847,6 +847,17 @@ def _check_like(name, new, old):
   return new.contiguous()
 
 
+def _fricloss_tables(dof_frictionloss: torch.Tensor, tendon_frictionloss: torch.Tensor):
+  """The dofs make_constraint checks for a friction-loss row, and the count of tendons it checks (the rows themselves follow each world's
+  values).  A per-world field (more than one entry) may be written in place at any time, so every dof / tendon is listed then; a shared
+  field lists the entries that are positive."""
+  fl = dof_frictionloss.detach().cpu().numpy().reshape(dof_frictionloss.shape[0], -1)
+  adr = np.arange(fl.shape[1]) if fl.shape[0] > 1 else np.nonzero((fl > 0).any(axis=0))[0]
+  tf = tendon_frictionloss.detach().cpu().numpy().reshape(max(tendon_frictionloss.shape[0], 1), -1) if tendon_frictionloss.numel() else np.zeros((1, 0))
+  ntenfric = tf.shape[1] if tf.shape[0] > 1 else int((tf > 0).any(axis=0).sum())
+  return adr.astype(np.int32), int(ntenfric)
+
+
 def _install_model_rebind(m: types.Model, L, arrays, ints):
   """Assignments to bound Model / Option / Statistic fields reach the C handle (ADVICE r1: they used to be silent no-ops)."""
   h = m._handle
@@ -866,6 +877,17 @@ def _install_model_rebind(m: types.Model, L, arrays, ints):
       m._keep.append(x)
       nb = int(x.shape[0]) if batchable and x.numel() > 0 else 1
       _lib.check(L.mjb_model_set_array_batched(h, name.encode(), x.data_ptr(), nb, int(x.numel() // max(nb, 1))))
+      if name in ("dof_frictionloss", "tendon_frictionloss"):  # the friction-loss rows follow the new values
+        adr, ntenfric = _fricloss_tables(value if name == "dof_frictionloss" else m.dof_frictionloss,
+                                         value if name == "tendon_frictionloss" else m.tendon_frictionloss)
+        a = _ptr_tensor(torch.from_numpy(adr).to(value.device))
+        m._keep.append(a)
+        _lib.check(L.mjb_model_set_array_batched(h, b"dof_fricloss_adr", a.data_ptr(), 1, int(a.numel())))
+        _lib.check(L.mjb_model_set_int(h, b"nfricdof", len(adr)))
+        _lib.check(L.mjb_model_set_int(h, b"ntenfric", ntenfric))
+        object.__setattr__(m, "dof_fricloss_adr", torch.from_numpy(adr).to(value.device))
+        object.__setattr__(m, "ntenfric", ntenfric)
+        m._tables["dof_fricloss_adr"] = adr
     elif name in ints and name in m.__dict__ and isinstance(m.__dict__[name], int):
       raise AttributeError(f"Model.{name} is a compiled size / table constant and cannot be reassigned; build a new Model with put_model")
     return value

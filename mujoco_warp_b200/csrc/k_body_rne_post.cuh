@@ -17,14 +17,17 @@
     __syncwarp();
     // ... connect / weld equalities between bodies (:1562; rows are ordered connect, weld, joint) and contacts (:1660), one after the
     // other in row / pool order so that the sums are reproducible; lanes 0-5 own the six components
+    // (rows at or past njmax do not exist: a block cut by njmax contributes the rows it has)
     const float* force = d.efc_force + wb * d.njmax;
+    const int ne_rows = min(d.ne[w], d.njmax);
+    auto fr = [&](int r) { return r < ne_rows ? force[r] : 0.f; };
 #pragma unroll 1
-    for (int e = 0; e < d.ne[w];) {
+    for (int e = 0; e < ne_rows;) {
       const int id = d.efc_id[wb * d.njmax + e], type = m.eq_type[id];
       if (type != EQ_CONNECT && type != EQ_WELD) break;
       const int nrow = type == EQ_CONNECT ? 3 : 6, b1 = m.eq_obj1id[id], b2 = m.eq_obj2id[id];
-      const v3 f = mk3(force[e], force[e + 1], force[e + 2]);
-      const v3 tq = type == EQ_WELD ? mk3(force[e + 3], force[e + 4], force[e + 5]) : mk3(0.f, 0.f, 0.f);
+      const v3 f = mk3(fr(e), fr(e + 1), fr(e + 2));
+      const v3 tq = type == EQ_WELD ? mk3(fr(e + 3), fr(e + 4), fr(e + 5)) : mk3(0.f, 0.f, 0.f);
       const float* data = m.eq_data + 11 * id;
       for (int side = 0; side < 2; side++) {
         const int b = side ? b2 : b1;

@@ -194,9 +194,11 @@ k_constraint(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDe
           if (lane == 0) efc_row(m, d, w, efcid, pos, pos, invweight, m.eq_solref + 2 * e, m.eq_solimp + 5 * e, 0.f, Jqvel, 0.f, CNSTR_EQUALITY, e);
           continue;
         }
-        const int nrow = type == EQ_CONNECT ? 3 : 6, efcid = nefc;
+        // every row of the block that fits below njmax is written (the reference skips a block that ends at or beyond njmax,
+        // constraint.py:228, :1039, which leaves rows the solver reads unwritten)
+        const int nrow = type == EQ_CONNECT ? 3 : 6, efcid = nefc, nfit = min(nrow, njmax - efcid);
         nefc += nrow; ne += nrow;
-        if (efcid >= njmax - nrow) continue;
+        if (nfit <= 0) continue;
         const int b1 = o1, b2 = o2;
         const v3 a1 = ld3(data), a2 = ld3(data + 3);  // connect: a1 in body1, a2 in body2; weld: data[0:3] is in body2's frame
         const v3 pos1 = ld3(d.xpos + (wb * nb + b1) * 3) + matvec(d.xmat + (wb * nb + b1) * 9, type == EQ_CONNECT ? a1 : a2);
@@ -221,8 +223,8 @@ k_constraint(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDe
               Jqvelr = Jqvelr + jdr * qv; Jdotvr0 = Jdotvr0 + (dr1 - dr2) * qv;
             }
           }
-          Jw[(size_t)(efcid + 0) * nvp + c] = jdp.x; Jw[(size_t)(efcid + 1) * nvp + c] = jdp.y; Jw[(size_t)(efcid + 2) * nvp + c] = jdp.z;
-          if (type == EQ_WELD) { Jw[(size_t)(efcid + 3) * nvp + c] = jdr.x; Jw[(size_t)(efcid + 4) * nvp + c] = jdr.y; Jw[(size_t)(efcid + 5) * nvp + c] = jdr.z; }
+#pragma unroll
+          for (int k = 0; k < 6; k++) if (k < nfit) Jw[(size_t)(efcid + k) * nvp + c] = comp3(k < 3 ? jdp : jdr, k < 3 ? k : k - 3);
         }
         Jqvelp = warp_sum3v(Jqvelp); Jdotvp = warp_sum3v(Jdotvp);
         const v3 cpos = pos1 - pos2;
@@ -240,7 +242,7 @@ k_constraint(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDe
           Jdotvr = (t1 + t2 + t3) * (0.5f * torquescale);
         }
         const float pos_imp = sqrtf(dot(cpos, cpos) + dot(crot, crot));
-        if (lane < nrow) {
+        if (lane < nfit) {
           const bool rot = lane >= 3;
           const int k = rot ? lane - 3 : lane;
           const float invw = rot ? m.body_invweight0[2 * b1 + 1] + m.body_invweight0[2 * b2 + 1] : invw_t;
@@ -252,19 +254,30 @@ k_constraint(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDe
     }
   }
 
-  // ---- dof friction loss rows (always present when frictionloss > 0)
+  // ---- dof friction loss rows: one per listed dof whose frictionloss is positive in this world (dof_fricloss_adr lists every dof when
+  // dof_frictionloss is per world), allocated in dof order by ballot / prefix like the joint limits
   if (!(m.disableflags & DSBL_FRICTIONLOSS)) {
-    nf = m.nfricdof;
-    for (int i = 0; i < nf; i++) {
-      const int efcid = nefc + i, dof = m.dof_fricloss_adr[i];
-      if (efcid >= njmax) break;
 #pragma unroll 1
-      for (int c = lane; c < nvp; c += 32) Jw[(size_t)efcid * nvp + c] = c == dof ? 1.0f : 0.f;
-      if (lane == 0)
-        efc_row(m, d, w, efcid, 0.f, 0.f, m.dof_invweight0[dof], m.dof_solref + 2 * dof, m.dof_solimp + 5 * dof, 0.f, qvel[dof],
-                m.dof_frictionloss[dof], CNSTR_FRICTION_DOF, dof);
+    for (int i0 = 0; i0 < m.nfricdof; i0 += 32) {
+      const int i = i0 + lane, dof = i < m.nfricdof ? m.dof_fricloss_adr[i] : 0;
+      const float fl = i < m.nfricdof ? m.dof_frictionloss[dof] : 0.f;
+      const unsigned bal = __ballot_sync(FULL_MASK, fl > 0.f);
+      const int efcid = nefc + __popc(bal & ((1u << lane) - 1u));
+      if (fl > 0.f && efcid < njmax)
+        efc_row(m, d, w, efcid, 0.f, 0.f, m.dof_invweight0[dof], m.dof_solref + 2 * dof, m.dof_solimp + 5 * dof, 0.f, qvel[dof], fl,
+                CNSTR_FRICTION_DOF, dof);
+      unsigned rem = bal;
+      while (rem) {  // whole warp writes each row's J
+        const int src = __ffs(rem) - 1;
+        rem &= rem - 1;
+        const int r = __shfl_sync(FULL_MASK, efcid, src), dcol = __shfl_sync(FULL_MASK, dof, src);
+        if (r < njmax)
+#pragma unroll 1
+          for (int c = lane; c < nvp; c += 32) Jw[(size_t)r * nvp + c] = c == dcol ? 1.0f : 0.f;
+      }
+      const int n = __popc(bal);
+      nefc += n; nf += n;
     }
-    nefc += nf;
     if (EQ && m.ntenfric > 0) {  // tendon friction loss (constraint.py:1867-1985)
 #pragma unroll 1
       for (int t = 0; t < m.ntendon; t++) {

@@ -16,6 +16,9 @@ namespace {
 //   contact rows      constraint.py:2728-2753 / :3100-3250  dof chains of the two (weld) bodies, descending dof, stopping at the first common dof
 //   connect / weld    :262-370 / :1130-1240                  union of the two chains, descending (common ancestors kept)
 //   joint equality    :570-606  dof1 [, dof2];   dof friction :1821  dof;   slide / hinge limit :2041  dof;   ball limit :2182  dof, dof + 1, dof + 2
+//   tendon friction / limit :1930 / :2315  the tendon's ten_J_colind entries, in their order (zeros kept)
+//   tendon equality   :741-800  ascending merge of the two tendons' ten_J_colind (the second only when the polynomial's slope is
+//                     nonzero): the whole merge is reserved, the entries whose value is nonzero are stored and counted in rownnz
 // Row addresses are the running sum of rownnz in row order (the reference hands them out with an atomic, i.e. in its launch order; run
 // sequentially that is the same sequence).  A row that does not fit in njmax_nnz raises OVF_NJMAX_NNZ and stays empty.
 __device__ __forceinline__ int chain_start(const ModelDev& m, int body) {
@@ -37,6 +40,21 @@ __device__ __forceinline__ int chain_walk(const ModelDev& m, int da1, int da2, b
   return n;
 }
 
+// ascending merge of the ten_J_colind rows of tendons t1 and t2 (t2 = -1: t1 alone); emit(col, k) per distinct column
+template <typename F>
+__device__ __forceinline__ int tendon_merge(const ModelDev& m, int t1, int t2, F emit) {
+  const int adr1 = m.ten_J_rowadr[t1], n1 = m.ten_J_rownnz[t1], adr2 = t2 > -1 ? m.ten_J_rowadr[t2] : 0, n2 = t2 > -1 ? m.ten_J_rownnz[t2] : 0;
+  int p1 = 0, p2 = 0, n = 0;
+  while (p1 < n1 || p2 < n2) {
+    const int c1 = p1 < n1 ? m.ten_J_colind[adr1 + p1] : INT_MAX, c2 = p2 < n2 ? m.ten_J_colind[adr2 + p2] : INT_MAX, c = min(c1, c2);
+    if (c1 == c) p1++;
+    if (c2 == c) p2++;
+    emit(c, n);
+    n++;
+  }
+  return n;
+}
+
 __global__ void __launch_bounds__(32)
 k_efc_csr(const __grid_constant__ ModelDev m, const __grid_constant__ DataDev d) {
   const int lane = threadIdx.x, w = blockIdx.x + d.w0;
@@ -51,27 +69,48 @@ k_efc_csr(const __grid_constant__ ModelDev m, const __grid_constant__ DataDev d)
 #pragma unroll 1
   for (int r0 = 0; r0 < nrow; r0 += 32) {
     const int r = r0 + lane;
-    int kind = 0, a1 = -1, a2 = -1, nnz = 0;  // kind 0: listed dofs a1 [, a2] / ball triple; 1: chain union; 2: chain difference
+    // kind 0: listed dofs a1 [, a2] / ball triple; 1: chain union; 2: chain difference; 4: tendon a1 [merged with tendon a2]; 5: tendon a1
+    int kind = 0, a1 = -1, a2 = -1, nnz = 0;
+    const float* Jr = Jd + (size_t)r * nvp;
     if (r < nrow) {
       const int type = d.efc_type[wb * njmax + r], id = d.efc_id[wb * njmax + r];
       if (type == CNSTR_EQUALITY) {
-        if (m.eq_type[id] == EQ_JOINT) { a1 = m.jnt_dofadr[m.eq_obj1id[id]]; a2 = m.eq_obj2id[id] > -1 ? m.jnt_dofadr[m.eq_obj2id[id]] : -1; nnz = a2 >= 0 ? 2 : 1; }
-        else { kind = 1; a1 = chain_start(m, m.eq_obj1id[id]); a2 = chain_start(m, m.eq_obj2id[id]); }
+        const int o1 = m.eq_obj1id[id], o2 = m.eq_obj2id[id];
+        if (m.eq_type[id] == EQ_JOINT) { a1 = m.jnt_dofadr[o1]; a2 = o2 > -1 ? m.jnt_dofadr[o2] : -1; nnz = a2 >= 0 ? 2 : 1; }
+        else if (m.eq_type[id] == EQ_TENDON) {
+          kind = 4; a1 = o1;
+          if (o2 > -1) {  // the polynomial's slope, as k_constraint evaluates it
+            const ModelDev mw = world_model(m, w, d.nworld);
+            const float* data = mw.eq_data + 11 * id;
+            const float dif = d.ten_length[wb * m.ntendon + o2] - mw.tendon_length0[o2], dif2 = dif * dif, dif3 = dif2 * dif;
+            if (data[1] + 2.0f * data[2] * dif + 3.0f * data[3] * dif2 + 4.0f * data[4] * dif3 != 0.f) a2 = o2;
+          }
+          nnz = tendon_merge(m, a1, a2, [](int, int) {});
+        } else { kind = 1; a1 = chain_start(m, o1); a2 = chain_start(m, o2); }
       } else if (type == CNSTR_FRICTION_DOF) { a1 = id; nnz = 1; }
       else if (type == CNSTR_LIMIT_JOINT) { a1 = m.jnt_dofadr[id]; if (m.jnt_type[id] == JNT_BALL) { kind = 3; nnz = 3; } else nnz = 1; }
+      else if (type == CNSTR_FRICTION_TENDON || type == CNSTR_LIMIT_TENDON) { kind = 5; a1 = id; nnz = m.ten_J_rownnz[id]; }
       else { kind = 2; a1 = chain_start(m, m.geom_bodyid[d.contact_geom[2 * (size_t)id]]); a2 = chain_start(m, m.geom_bodyid[d.contact_geom[2 * (size_t)id + 1]]); }
       if (kind == 1 || kind == 2) nnz = chain_walk(m, a1, a2, kind == 2, [](int, int) {});
     }
     const int adr = base + warp_excl_scan(nnz, lane);
     base += warp_sum_i(nnz);
     if (r < nrow) {
-      d.efc_J_rownnz[wb * njmax + r] = nnz;
+      if (kind == 4) {  // rownnz counts the stored (nonzero) entries of the reserved merge; a row that does not fit keeps no rownnz (:758-760)
+        int k = 0;
+        if (adr + nnz <= d.njmax_nnz) {
+          tendon_merge(m, a1, a2, [&](int c, int) { if (Jr[c] != 0.f) { col[adr + k] = c; Jv[adr + k] = Jr[c]; k++; } });
+          d.efc_J_rownnz[wb * njmax + r] = k;
+        }
+      } else {
+        d.efc_J_rownnz[wb * njmax + r] = nnz;
+      }
       if (adr + nnz > d.njmax_nnz) { ovf = true; continue; }
       d.efc_J_rowadr[wb * njmax + r] = adr;
-      const float* Jr = Jd + (size_t)r * nvp;
       if (kind == 1 || kind == 2) chain_walk(m, a1, a2, kind == 2, [&](int da, int k) { col[adr + k] = da; Jv[adr + k] = Jr[da]; });
       else if (kind == 3) { for (int k = 0; k < 3; k++) { col[adr + k] = a1 + k; Jv[adr + k] = Jr[a1 + k]; } }
-      else { col[adr] = a1; Jv[adr] = Jr[a1]; if (nnz == 2) { col[adr + 1] = a2; Jv[adr + 1] = Jr[a2]; } }
+      else if (kind == 5) { for (int k = 0; k < nnz; k++) { const int c = m.ten_J_colind[m.ten_J_rowadr[a1] + k]; col[adr + k] = c; Jv[adr + k] = Jr[c]; } }
+      else if (kind == 0) { col[adr] = a1; Jv[adr] = Jr[a1]; if (nnz == 2) { col[adr + 1] = a2; Jv[adr + 1] = Jr[a2]; } }
     }
   }
   if (__any_sync(FULL_MASK, ovf) && lane == 0) d.overflow[w] |= OVF_NJMAX_NNZ;
