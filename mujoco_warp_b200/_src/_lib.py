@@ -15,7 +15,7 @@ _PKG = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 _CSRC = os.path.join(_PKG, "csrc")
 LIB_PATH = os.environ.get("MJB_LIB", os.path.join(_PKG, "libmjb200.so"))  # MJB_LIB: A/B-test an alternative build
 HEADER_PATH = os.path.join(os.path.dirname(_PKG), "include", "mjb200.h")
-SOURCES = ["capi.cu", "k_position.cu", "k_collision.cu", "k_collision_mesh.cu", "k_collision_mesh_large.cu", "k_constraint.cu", "k_velocity.cu", "k_solver.cu", "k_integrate.cu", "k_implicit.cu", "k_support.cu", "k_sensor.cu", "k_sensor_collision.cu", "k_sensor_collision_large.cu", "k_sensor_contact.cu", "k_ray.cu", "k_inverse.cu", "k_set_const.cu", "k_energy.cu", "k_history.cu", "k_render.cu", "k_body_stages.cu"]
+SOURCES = ["capi.cu", "k_position.cu", "k_collision.cu", "k_collision_mesh.cu", "k_collision_mesh_large.cu", "k_constraint.cu", "k_velocity.cu", "k_solver.cu", "k_integrate.cu", "k_implicit.cu", "k_support.cu", "k_sensor.cu", "k_sensor_collision.cu", "k_sensor_collision_large.cu", "k_sensor_contact.cu", "k_sensor_rangefinder.cu", "k_ray.cu", "k_inverse.cu", "k_set_const.cu", "k_energy.cu", "k_history.cu", "k_render.cu", "k_body_stages.cu"]
 NVCC_FLAGS = ["-std=c++17", "-O3", "-lineinfo", "-gencode", "arch=compute_90a,code=sm_90a", "--extended-lambda", "-Xcompiler", "-fPIC", "-shared"]
 
 _lib = None

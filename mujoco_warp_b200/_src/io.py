@@ -54,6 +54,9 @@ _EXTRA_SENSORS = {
   C.SENS_INSIDESITE: ((C.OBJ_BODY, C.OBJ_XBODY, C.OBJ_GEOM, C.OBJ_SITE, C.OBJ_CAMERA), (C.OBJ_SITE,)),
   **{t: ((C.OBJ_TENDON,), None) for t in (C.SENS_TENDONLIMITPOS, C.SENS_TENDONLIMITVEL, C.SENS_TENDONLIMITFRC, C.SENS_TENDONACTFRC)},
 }
+# every sensor type put_model checks the object kinds of: the EXTRA ones and the rangefinder, which its own kernel runs (a site's z axis,
+# one output: MuJoCo's camera-attached and multi-output rangefinders are refused)
+_CHECKED_SENSORS = {**_EXTRA_SENSORS, C.SENS_RANGEFINDER: ((C.OBJ_SITE,), None)}
 _SIZES = ["nq", "nv", "nu", "na", "nbody", "njnt", "ngeom", "nsite", "ncam", "nlight", "ntree", "nkey", "nmocap", "neq", "ntendon", "nflex"]
 
 _SUPPORTED_PAIRS = {
@@ -466,8 +469,9 @@ def _contact_sensor_intprm(mjm) -> np.ndarray:
 
 
 def _validate_extra_sensors(mjm):
-  """Checks the object kinds and ids of the magnetometer / camprojection / insidesite / tendon sensors again, for models that did not come
-  from this package's compiler.  Returns whether the model has one (k_sensor's EXTRA build)."""
+  """Checks the object kinds and ids of the magnetometer / camprojection / insidesite / tendon sensors and the rangefinders (and that each
+  rangefinder has one output) again, for models that did not come from this package's compiler.  Returns whether the model has one of the
+  first kinds (k_sensor's EXTRA build); a rangefinder does not select it."""
   ns = int(getattr(mjm, "nsensor", 0))
   stype = np.asarray(mjm.sensor_type).reshape(ns) if ns else np.zeros(0, dtype=int)
   counts = {C.OBJ_BODY: int(mjm.nbody), C.OBJ_XBODY: int(mjm.nbody), C.OBJ_GEOM: int(mjm.ngeom), C.OBJ_SITE: int(getattr(mjm, "nsite", 0)),
@@ -475,12 +479,14 @@ def _validate_extra_sensors(mjm):
   names = getattr(getattr(mjm, "names", None), "sensor", None)
   found = False
   for s in range(ns):
-    if int(stype[s]) not in _EXTRA_SENSORS:
+    if int(stype[s]) not in _CHECKED_SENSORS:
       continue
-    found = True
+    found |= int(stype[s]) in _EXTRA_SENSORS
     what = f"sensor {s}" + (f" ('{names[s]}')" if names is not None and s < len(names) else "")
-    for side, kinds, typ, oid in (("object", _EXTRA_SENSORS[int(stype[s])][0], int(mjm.sensor_objtype[s]), int(mjm.sensor_objid[s])),
-                                  ("reference", _EXTRA_SENSORS[int(stype[s])][1], int(getattr(mjm, "sensor_reftype", np.zeros(ns))[s]),
+    if int(stype[s]) == C.SENS_RANGEFINDER and int(mjm.sensor_dim[s]) != 1:
+      raise ValueError(f"{what}: a rangefinder has one output here, got dim {int(mjm.sensor_dim[s])}")
+    for side, kinds, typ, oid in (("object", _CHECKED_SENSORS[int(stype[s])][0], int(mjm.sensor_objtype[s]), int(mjm.sensor_objid[s])),
+                                  ("reference", _CHECKED_SENSORS[int(stype[s])][1], int(getattr(mjm, "sensor_reftype", np.zeros(ns))[s]),
                                    int(getattr(mjm, "sensor_refid", -np.ones(ns))[s]))):
       if kinds is None:
         continue
@@ -489,6 +495,24 @@ def _validate_extra_sensors(mjm):
       if not 0 <= oid < counts[typ]:
         raise ValueError(f"{what}: {side} names an unknown object (id {oid})")
   return found
+
+
+def rangefinder_tables(mjm) -> dict:
+  """The reference's rangefinder fields (io.py:442, :885-887, :910): nrangefinder, the sensor id of each rangefinder, the rangefinder id of
+  each sensor (-1 for the others) and the body of each rangefinder's site, which its ray excludes."""
+  ns = int(getattr(mjm, "nsensor", 0))
+  stype = np.asarray(mjm.sensor_type).reshape(ns) if ns else np.zeros(0, dtype=int)
+  adr = np.nonzero(stype == C.SENS_RANGEFINDER)[0].astype(np.int32)
+  rsa = np.full(ns, -1, dtype=np.int32)
+  rsa[adr] = np.arange(len(adr), dtype=np.int32)
+  body = np.asarray(mjm.site_bodyid).astype(np.int32)[np.asarray(mjm.sensor_objid).reshape(ns)[adr]] if len(adr) else np.zeros(0, dtype=np.int32)
+  return dict(nrangefinder=len(adr), sensor_rangefinder_adr=adr, rangefinder_sensor_adr=rsa, sensor_rangefinder_bodyid=body)
+
+
+def check_rangefinder_worlds(nworld: int, nrangefinder: int):
+  """The rangefinder kernel indexes (world, rangefinder) pairs with an int, as mjb_rays does its rays."""
+  if nworld * nrangefinder > 0x7FFFFFFF:
+    raise ValueError(f"nworld * nrangefinder = {nworld} * {nrangefinder} exceeds the int range")
 
 
 def _validate_history(mjm):
@@ -682,6 +706,11 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
   stype = np.asarray(mjm.sensor_type) if nsensor else np.zeros(0, dtype=int)
   m.sensor_subtree_vel = bool(np.isin(stype, (C.SENS_SUBTREELINVEL, C.SENS_SUBTREEANGMOM)).any())  # reference io.py:896-897
   m.sensor_extra = _validate_extra_sensors(mjm)
+  # rangefinders (reference io.py:442, :885-887, :910): one kernel after k_sensor writes their slots (k_sensor skips them)
+  rft = rangefinder_tables(mjm)
+  m.nrangefinder = rft.pop("nrangefinder")
+  for n, x in rft.items():
+    setattr(m, n, dev_i(x))
   m.sensor_rne_postconstraint = bool(np.isin(stype, (C.SENS_ACCELEROMETER, C.SENS_FORCE, C.SENS_TORQUE, C.SENS_FRAMELINACC, C.SENS_FRAMEANGACC)).any())  # :900
   # <contact> sensors (reference io.py:409-413, :441, :898): their ids, [dataspec, reduce, num] per sensor, and the match capacity
   sensor_intprm = _contact_sensor_intprm(mjm)
@@ -789,7 +818,7 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
                ("nsensorcollision_ccd", m.nsensorcollision_ccd), ("nsensor_energy", len(t["sensor_energy_adr"])),
                ("sensor_e_potential", m.sensor_e_potential), ("sensor_e_kinetic", m.sensor_e_kinetic),
                ("nsensorcontact", m.nsensorcontact), ("contact_sensor_maxmatch", m.opt.contact_sensor_maxmatch), ("nhistory", m.nhistory), ("nactuator_history", int((hf["actuator_history"][:, 0] > 0).sum())), ("nsensor_history", len(m.sensor_history_id)),
-               ("npolygonmax", m.npolygonmax), ("nmeshdegmax", m.nmeshdegmax), ("sensor_extra", int(m.sensor_extra))):
+               ("npolygonmax", m.npolygonmax), ("nmeshdegmax", m.nmeshdegmax), ("sensor_extra", int(m.sensor_extra)), ("nrangefinder", m.nrangefinder)):
     _lib.check(L.mjb_model_set_int(h, k.encode(), int(v)))
   g = np.asarray(o.gravity, dtype=np.float64)
   floats = dict(timestep=o.timestep, tolerance=tol, ls_tolerance=o.ls_tolerance, impratio_invsqrt=1.0 / np.sqrt(o.impratio),
@@ -817,7 +846,7 @@ def put_model(mjm, batch_sizes=None) -> types.Model:
                                          "geom_fluid", "body_fluid", "body_geomadr", "body_geomnum", "sensor_collision_start_adr", "sensor_collision_pair",
                                          "sensor_collision_id", "sensor_collision_adr", "sensor_collision_flip", "actuator_acc0", "actuator_lengthrange", "jnt_limited", "sensor_energy_adr",
                                          "actuator_history", "actuator_historyadr", "actuator_delay", "sensor_history", "sensor_historyadr", "sensor_delay",
-                                         "sensor_interval", "sensor_history_id", "sensor_contact_adr", "sensor_intprm",
+                                         "sensor_interval", "sensor_history_id", "sensor_contact_adr", "sensor_intprm", "sensor_rangefinder_adr", "sensor_rangefinder_bodyid",
                                          "cam_fovy", "cam_intrinsic", "cam_sensorsize", "cam_resolution"]
                                         + [n for n, _ in _TENDON_FLOATS]):
     dev_names.setdefault(n, getattr(m, n))
@@ -1028,6 +1057,7 @@ def make_data(mjm, nworld: int = 1, nconmax=None, nccdmax=None, njmax=None, njma
     raise ValueError("nworld must be >= 1")
   if nconmax < 0 or njmax < 0:
     raise ValueError("nconmax and njmax must be >= 0")
+  check_rangefinder_worlds(nworld, m.nrangefinder)
   naconmax = nworld * nconmax if naconmax is None else int(naconmax)
   njmax_pad, nv_pad = _get_padded_sizes(m.nv, njmax, False)
   if m.is_sparse:

@@ -15,6 +15,7 @@ struct mjbModel {
   FluidDev fluid;  // qfrc_fluid stays null here: it is the Data's (fluid() below)
   SensorCollisionDev sc;
   SensorContactDev scon;  // the <contact> sensors and Option.contact_sensor_maxmatch
+  RangefinderDev rf;      // the rangefinder sensors
   SetConstDev setc;  // actuator_acc0 and the meaninertia output, bound by name; qpos_save stays null here (the Data's)
   EnergyDev en;      // the energy sensors; energy stays null here (the Data's: energy() below)
   HistoryDev hist;   // the delay fields; history and ctrl_delayed stay null here (the Data's: history() below)
@@ -79,6 +80,7 @@ mjbModel* mjb_model_create(void) {
   memset(&m->fluid, 0, sizeof(FluidDev));
   memset(&m->sc, 0, sizeof(SensorCollisionDev));
   memset(&m->scon, 0, sizeof(SensorContactDev));
+  memset(&m->rf, 0, sizeof(RangefinderDev));
   memset(&m->setc, 0, sizeof(SetConstDev));
   memset(&m->en, 0, sizeof(EnergyDev));
   memset(&m->hist, 0, sizeof(HistoryDev));
@@ -107,6 +109,9 @@ int mjb_model_set_int(mjbModel* m, const char* name, int v) {
     return 0;
   }
   if (!strcmp(name, "nsensorcontact")) { m->scon.nsensorcontact = v; return 0; }
+#define X(n) if (!strcmp(name, #n)) { m->rf.n = v; return 0; }
+  MJB_RANGEFINDER_INTS(X)
+#undef X
   if (!strcmp(name, "sensor_extra")) { m->dev.sensor_extra = v; return 0; }
 #define X(n) if (!strcmp(name, #n)) { m->en.n = v; return 0; }
   MJB_ENERGY_INTS(X)
@@ -142,6 +147,9 @@ int mjb_model_set_array_batched(mjbModel* m, const char* name, const void* p, in
 #undef X
 #define X(n) if (!strcmp(name, #n)) { if (nbatch != 1) return fail(std::string("shared by all worlds (not batched): ") + name); m->scon.n = (const int*)p; return 0; }
   MJB_SENSCON_IARRS(X)
+#undef X
+#define X(n) if (!strcmp(name, #n)) { if (nbatch != 1) return fail(std::string("shared by all worlds (not batched): ") + name); m->rf.n = (const int*)p; return 0; }
+  MJB_RANGEFINDER_IARRS(X)
 #undef X
 #define X(n) if (!strcmp(name, #n)) { if (nbatch != 1) return fail(std::string("shared by all worlds (not batched): ") + name); m->en.n = (const int*)p; return 0; }
   MJB_ENERGY_IARRS(X)
@@ -193,6 +201,9 @@ int mjb_model_finalize(mjbModel* m) {
   MJB_SENSCON_IARRS(X)
 #undef X
   if (m->scon.contact_sensor_maxmatch < 1) return fail("model int not set: contact_sensor_maxmatch");
+#define X(n) if (!m->rf.n) return fail(std::string("model array not set: ") + #n);
+  MJB_RANGEFINDER_IARRS(X)
+#undef X
 #define X(n) if (!m->en.n) return fail(std::string("model array not set: ") + #n);
   MJB_ENERGY_IARRS(X)
 #undef X
@@ -474,8 +485,8 @@ int mjb_render_rays(const mjbRender* rc, float* ray, void* stream) {
 }
 // The k_energy parts of the position-stage sensors (sensor.py:845-849): the terms the energy sensors read, and the sensors themselves
 // The sensors of `stages` (1 pos, 2 vel, 4 acc) for dd's world range: k_sensor (with the collision sensors for the position stage), then
-// for the acceleration stage the <contact> sensors (sensor.py:2605-2658), which read the solver's efc_force.  A model without contact
-// sensors launches what it launched before they existed.
+// for the position stage the rangefinders (sensor.py:815-843), and for the acceleration stage the <contact> sensors (sensor.py:2605-2658),
+// which read the solver's efc_force.  A model without rangefinders or contact sensors launches what it launched before they existed.
 static cudaError_t sensors(const mjbModel* m, const mjbData* d, const DataDev& dd, int stages, cudaStream_t s) {
   cudaError_t e;
   if (mesh_large(m) && m->sc.nsensorcollision > 0) {  // the collision sensors run the CCD_MESH = 2 build, after k_sensor as launch_sensor orders them
@@ -486,6 +497,7 @@ static cudaError_t sensors(const mjbModel* m, const mjbData* d, const DataDev& d
   } else {
     e = launch_sensor(m->dev, dd, stages, s, m->sc);
   }
+  if (e == cudaSuccess && m->rf.nrangefinder > 0 && (stages & 1) && !(m->dev.disableflags & DSBL_SENSOR)) e = launch_sensor_rangefinder(m->dev, dd, m->rf, s);
   if (e != cudaSuccess || m->dev.nsensor == 0 || !(stages & 4) || m->scon.nsensorcontact == 0 || (m->dev.disableflags & DSBL_SENSOR)) return e;
   return launch_sensor_contact(m->dev, dd, m->scon, s);
 }

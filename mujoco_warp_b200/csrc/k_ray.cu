@@ -2,10 +2,11 @@
 //
 // Replaces (reference, /root/reference/mujoco_warp/_src/): ray.py:1219 rays / :907 _ray without a render context (no BVH).
 // One thread per (world, ray) pair, flattened world-major (i = w * nray + r), so the three outputs are written coalesced.  Every
-// thread scans the geoms in ascending order: the loop index is warp-uniform, so the geom-type switch and the model-constant loads
-// do not diverge, and the lanes of one world read the same geom_xpos / geom_xmat address (one broadcast load).  The closest hit
-// is replaced only on a strictly smaller distance, so ties go to the lowest geom id, as the reference's argmin within a tile and
-// strict compare across tiles do (ray.py:994-1004); a ray's result does not depend on scheduling.
+// thread scans the geoms in ascending order (mjb_ray.cuh ray_scan, shared with the rangefinder sensor): the loop index is
+// warp-uniform, so the geom-type switch and the model-constant loads do not diverge, and the lanes of one world read the same
+// geom_xpos / geom_xmat address (one broadcast load).  The closest hit is replaced only on a strictly smaller distance, so ties go
+// to the lowest geom id, as the reference's argmin within a tile and strict compare across tiles do (ray.py:994-1004); a ray's
+// result does not depend on scheduling.
 #include "mjb_launch.cuh"
 #include "mjb_ray.cuh"
 
@@ -28,36 +29,11 @@ k_ray(const __grid_constant__ ModelDev mp, const __grid_constant__ DataDev d, co
   const size_t src = (size_t)(pnt_nbatch == 1 ? 0 : w) * nray + r;
   const v3 p = live ? ld3(pnt + 3 * src) : ray_zero3(), v = live ? ld3(vec + 3 * src) : ray_zero3();
   const int bx = live ? bodyexclude[r] : -1;
-  const float* xpos = d.geom_xpos + (size_t)w * m.ngeom * 3;
-  const float* xmat = d.geom_xmat + (size_t)w * m.ngeom * 9;
-
-  float best = MJ_MAXVAL;
-  int best_g = -1;
-  v3 best_n = ray_zero3();
-#pragma unroll 1
-  for (int g = 0; g < m.ngeom; g++) {
-    const bool skip = !live || ray_eliminate(m, g, filter, bx);
-    const int type = m.geom_type[g];
-    const v3 pos = ld3(xpos + 3 * g), size = ld3(m.geom_size + 3 * g);
-    const float* mat = xmat + 9 * g;
-    float x = -1.f;
-    v3 n = ray_zero3();
-    if (MESH && type == GEOM_MESH) {
-      // ray.py:646 bounding-box test; the warp skips the triangles when no lane's ray enters the box
-      const bool inbox = !skip && ray_box<false>(pos, mat, size, p, v, nullptr) >= 0.f;
-      if (__any_sync(FULL_MASK, inbox) && inbox) {
-        const int id = m.geom_dataid[g];
-        int f0, f1;
-        ray_mesh_range(m, id, &f0, &f1);
-        x = ray_mesh_faces(m.mesh_face, f0, f1, m.mesh_vert + 3 * m.mesh_vertadr[id], pos, mat, p, v, &n);
-      }
-    } else if (!skip) {
-      x = ray_geom<true>(pos, mat, size, p, v, type, &n);
-    }
-    if (x >= 0.f && x < best) { best = x; best_g = g; best_n = n; }
-  }
+  int best_g;
+  v3 best_n;
+  const float best = ray_scan<MESH>(m, d.geom_xpos + (size_t)w * m.ngeom * 3, d.geom_xmat + (size_t)w * m.ngeom * 9, filter, bx, live, p, v, &best_g, &best_n);
   if (!live) return;
-  dist_out[i] = best_g >= 0 ? best : -1.f;
+  dist_out[i] = best;
   geomid_out[i] = best_g;
   st3(normal_out + 3 * (size_t)i, best_n);
 }

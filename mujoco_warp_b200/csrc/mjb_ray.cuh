@@ -1,4 +1,5 @@
-// mjb_ray.cuh -- intersection of one ray with one geom (fp32), shared by k_ray (mjw.ray / mjw.rays) and the touch sensor (k_sensor).
+// mjb_ray.cuh -- intersection of one ray with one geom (fp32), and the closest-hit scan over a world's geoms, shared by k_ray (mjw.ray / mjw.rays),
+// the rangefinder sensor (k_sensor_rangefinder) and the touch sensor (k_sensor).
 //
 // Restates the reference's ray.py (/root/reference/mujoco_warp/_src/ray.py) in its operation order: :33 _ray_map, :53 _ray_eliminate,
 // :106 _ray_quad, :129 _orthogonal_basis, :155 _ray_triangle, :214 ray_plane, :238 ray_sphere, :255 ray_capsule, :329 ray_ellipsoid,
@@ -261,4 +262,51 @@ static __device__ __forceinline__ float ray_world_geom(const ModelDev& m, const 
   const float* mat = geom_xmat + 9 * g;
   if (m.geom_type[g] == GEOM_MESH) return ray_mesh(m, m.geom_dataid[g], pos, mat, size, pnt, vec, normal);
   return ray_geom<true>(pos, mat, size, pnt, vec, m.geom_type[g], normal);
+}
+
+// The warp vote of the scan below; compiled as host C++ each ray is its own warp
+static __device__ __forceinline__ bool ray_warp_any(bool v) {
+#ifdef __CUDA_ARCH__
+  return __any_sync(FULL_MASK, v);
+#else
+  return v;
+#endif
+}
+
+// :907 _ray's closest-hit scan for one ray of world geoms (geom_xpos / geom_xmat of the world), shared by k_ray and k_sensor_rangefinder.
+// Every lane of the warp must call it (`live` false for lanes past the last ray, which keep the warp-wide vote of the mesh path
+// complete): geoms are visited in ascending order and the closest hit is replaced only on a strictly smaller distance, so ties go to
+// the lowest geom id.  Returns the distance (-1 on a miss), with the geom id (-1) and world-frame normal (zero) of the hit.
+// MESH: the model has meshes (the triangle path is compiled in); `m` is the model as the ray's world sees it.
+template <bool MESH>
+static __device__ __forceinline__ float ray_scan(const ModelDev& m, const float* xpos, const float* xmat, const RayFilter& filter, int bodyexclude, bool live,
+                                                 v3 p, v3 v, int* geomid, v3* normal) {
+  float best = MJ_MAXVAL;
+  int best_g = -1;
+  v3 best_n = ray_zero3();
+#pragma unroll 1
+  for (int g = 0; g < m.ngeom; g++) {
+    const bool skip = !live || ray_eliminate(m, g, filter, bodyexclude);
+    const int type = m.geom_type[g];
+    const v3 pos = ld3(xpos + 3 * g), size = ld3(m.geom_size + 3 * g);
+    const float* mat = xmat + 9 * g;
+    float x = -1.f;
+    v3 n = ray_zero3();
+    if (MESH && type == GEOM_MESH) {
+      // ray.py:646 bounding-box test; the warp skips the triangles when no lane's ray enters the box
+      const bool inbox = !skip && ray_box<false>(pos, mat, size, p, v, nullptr) >= 0.f;
+      if (ray_warp_any(inbox) && inbox) {
+        const int id = m.geom_dataid[g];
+        int f0, f1;
+        ray_mesh_range(m, id, &f0, &f1);
+        x = ray_mesh_faces(m.mesh_face, f0, f1, m.mesh_vert + 3 * m.mesh_vertadr[id], pos, mat, p, v, &n);
+      }
+    } else if (!skip) {
+      x = ray_geom<true>(pos, mat, size, p, v, type, &n);
+    }
+    if (x >= 0.f && x < best) { best = x; best_g = g; best_n = n; }
+  }
+  *geomid = best_g;
+  *normal = best_n;
+  return best_g >= 0 ? best : -1.f;
 }

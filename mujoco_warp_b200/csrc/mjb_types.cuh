@@ -169,6 +169,17 @@ struct SensorContactDev {
   const int* __restrict__ sensor_intprm;       // (nsensor, 3) dataspec, reduce, num of each contact sensor; zeros for the others
 };
 
+// ---------------------------------------------------------------- rangefinders (k_sensor_rangefinder.cu)
+// The rangefinder tables (reference io.py:885-887, :910), passed as one extra argument to k_sensor_rangefinder only, for the same reason
+// as FluidDev.  k_sensor skips the rangefinders' slots; this kernel writes them.
+#define MJB_RANGEFINDER_INTS(X) X(nrangefinder)
+#define MJB_RANGEFINDER_IARRS(X) X(sensor_rangefinder_adr) X(sensor_rangefinder_bodyid)
+struct RangefinderDev {
+  int nrangefinder;                                   // rangefinder sensors
+  const int* __restrict__ sensor_rangefinder_adr;     // (nrangefinder) their sensor ids
+  const int* __restrict__ sensor_rangefinder_bodyid;  // (nrangefinder) the body of each one's site (excluded from its ray)
+};
+
 // ---------------------------------------------------------------- set_const (k_set_const.cu)
 // The fields of mjb_set_const that are neither in ModelDev nor in DataDev, passed as one extra argument to its kernels only, for the
 // same reason as FluidDev.  Writes to the other derived Model fields go through ModelDev's pointers and nb_* / bs_*.
@@ -247,7 +258,7 @@ enum { EQ_CONNECT = 0, EQ_WELD = 1, EQ_JOINT = 2, EQ_TENDON = 3 };
 enum { TRN_JOINT = 0, TRN_TENDON = 3 };
 enum { OBJ_BODY = 1, OBJ_XBODY = 2, OBJ_GEOM = 5, OBJ_SITE = 6, OBJ_CAMERA = 7 };
 // mjtSensor values of the sensor types carried here (MuJoCo order, as in _src/constants.py)
-enum { SENS_TOUCH = 0, SENS_ACCELEROMETER = 1, SENS_VELOCIMETER = 2, SENS_GYRO = 3, SENS_FORCE = 4, SENS_TORQUE = 5, SENS_MAGNETOMETER = 6, SENS_CAMPROJECTION = 8, SENS_JOINTPOS = 9, SENS_JOINTVEL = 10, SENS_TENDONPOS = 11, SENS_TENDONVEL = 12, SENS_ACTUATORPOS = 13, SENS_ACTUATORVEL = 14,
+enum { SENS_TOUCH = 0, SENS_ACCELEROMETER = 1, SENS_VELOCIMETER = 2, SENS_GYRO = 3, SENS_FORCE = 4, SENS_TORQUE = 5, SENS_MAGNETOMETER = 6, SENS_RANGEFINDER = 7, SENS_CAMPROJECTION = 8, SENS_JOINTPOS = 9, SENS_JOINTVEL = 10, SENS_TENDONPOS = 11, SENS_TENDONVEL = 12, SENS_ACTUATORPOS = 13, SENS_ACTUATORVEL = 14,
        SENS_ACTUATORFRC = 15, SENS_JOINTACTFRC = 16, SENS_TENDONACTFRC = 17, SENS_BALLQUAT = 18, SENS_BALLANGVEL = 19, SENS_JOINTLIMITPOS = 20, SENS_JOINTLIMITVEL = 21, SENS_JOINTLIMITFRC = 22, SENS_TENDONLIMITPOS = 23,
        SENS_TENDONLIMITVEL = 24, SENS_TENDONLIMITFRC = 25, SENS_FRAMEPOS = 26, SENS_FRAMEQUAT = 27, SENS_FRAMEXAXIS = 28,
        SENS_FRAMEYAXIS = 29, SENS_FRAMEZAXIS = 30, SENS_FRAMELINVEL = 31, SENS_FRAMEANGVEL = 32, SENS_FRAMELINACC = 33, SENS_FRAMEANGACC = 34, SENS_SUBTREECOM = 35, SENS_SUBTREELINVEL = 36, SENS_SUBTREEANGMOM = 37, SENS_INSIDESITE = 38, SENS_GEOMDIST = 39, SENS_GEOMNORMAL = 40,
@@ -306,6 +317,8 @@ cudaError_t launch_contact_force(const ModelDev& m, const DataDev& d, const int*
 // the <contact> sensors of d's world range, after the acceleration-stage sensors (k_sensor_contact.cu)
 cudaError_t launch_sensor_contact(const ModelDev& m, const DataDev& d, const SensorContactDev& c, cudaStream_t s);
 size_t smem_sensor_contact(const SensorContactDev& c);
+// the rangefinders of d's world range, after k_sensor's position stage (k_sensor_rangefinder.cu)
+cudaError_t launch_sensor_rangefinder(const ModelDev& m, const DataDev& d, const RangefinderDev& r, cudaStream_t s);
 // inverse dynamics at the given d.qacc into qfrc_inverse (nworld, nv); disc: d.qacc is a discrete-time acceleration, converted first,
 // and the continuous one goes to qacc_cont (nworld, nv) (k_inverse.cu)
 cudaError_t launch_inverse(const ModelDev& m, const DataDev& d, float* qfrc_inverse, float* qacc_cont, bool disc, cudaStream_t s, const FluidDev& f);
